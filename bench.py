@@ -70,7 +70,25 @@ def parse_args(argv=None):
     ap.add_argument("--exchange", default="p2p", choices=["p2p", "nccl"], help="N>1: in-kernel peer-memory exchange (default) or host loop + NCCL all-reduce per batch")
     ap.add_argument("--ref-iterations", type=int, default=-1, help="NM iterations per reference-arm step (bounded sample); -1 = per-config default")
     ap.add_argument("--grid-poses", type=int, default=16384, help="C5: poses of the grid (16384 = the BASELINE figure)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float64; inputs are seeded, so runs compare output for output)")
     return ap.parse_args(argv)
+
+
+def dump_outputs(directory, outputs, limit=64 << 20):
+    """Writes every array of `outputs` as <directory>/<name>.npy in float64.  A step's outputs are normally far below
+    `limit` (one pose, simplex vertex and cost per solve, or one NID per grid pose); above it, every array keeps the same
+    fixed, seeded sample of its rows (seed 0, sorted) and <name>_rows.npy records which rows were kept."""
+    os.makedirs(directory, exist_ok=True)
+    arrays = {name: np.asarray(v, dtype=np.float64) for name, v in outputs.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    for name, a in arrays.items():
+        if total > limit and a.ndim > 0 and a.shape[0] > 1:
+            keep = max(1, int(a.shape[0] * limit / (2 * total)))  # half the budget for the samples, the rest covers the row lists
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], keep, replace=False))
+            a = a[rows]
+            np.save(os.path.join(directory, f"{name}_rows.npy"), rows.astype(np.float64))
+        np.save(os.path.join(directory, f"{name}.npy"), a)
 
 
 def start_poses(cfg, T_gt, count):
@@ -114,7 +132,7 @@ def config_dict(args, world, n_points, W, H):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     FIELDS = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -171,19 +189,7 @@ def measured_hbm_peak():
             return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def committed_ncu(config):
-    """Figures that only a profiler capture gives (DRAM traffic, executed instructions), read from the committed summary of
-    THIS config's capture (profiles/r02_ncu_<config>.json, written by tools/ncu_summary.py); None if not captured."""
-    path = os.path.join(ROOT, "profiles", f"r02_ncu_{config}.json")
-    if os.path.exists(path):
-        try:
-            return json.load(open(path))
-        except Exception:
-            pass
-    return None
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s)"
 
 
 def oracle_objects(bag):
@@ -351,8 +357,7 @@ def rank_cpus(ordered, siblings_of, local_rank, world):
 def bind_rank_to_cores(local_rank, world):
     """One slice of the host's cores per rank, NUMA node by NUMA node, whole physical cores (what `numactl` does for a
     launcher): the e2e path converts and uploads 200 MB of host doubles per solve at C3, and with every rank's pages and
-    conversion threads on whichever node the scheduler picked, two ranks ran that at 2.7x the single-rank time
-    (profiles/r02_bench_e_c3_n2.json; 1.2x with the binding, r02_bench_k_c3_n2.json).
+    conversion threads on whichever node the scheduler picked, the ranks contend for one node's memory bandwidth.
     Returns a description for the JSON line (None when nothing was changed)."""
     if world <= 1 or not hasattr(os, "sched_setaffinity"):
         return None
@@ -489,7 +494,7 @@ def main():
     if px is not None:
         cost.attach_peer_exchange(px)
         px.set_default(True)  # cost objects built inside the e2e call attach it too
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2 of an H100
 
     def barrier():
         if world > 1:
@@ -502,16 +507,19 @@ def main():
 
             nid = IG.score_poses(cost, grid, rank, world)
             mine = len(grid[rank::world])
-            return {"evals": len(grid) / world, "computed": mine, "batches": (mine + 7) // 8, "result": float(np.nanmin(nid))}
+            return {"evals": len(grid) / world, "computed": mine, "batches": (mine + 7) // 8, "result": float(np.nanmin(nid)), "outputs": {"grid_nid": nid}}
         ev = cm = bt = 0
         y = None
+        out = {"T_camera_lidar": [], "nm_x": [], "nm_cost": [], "nm_iterations": []}
         for T0 in starts:
-            _, r = VC.estimate_pose_on_costs([cost], T0, params, allreduce=ar)
+            T, r = VC.estimate_pose_on_costs([cost], T0, params, allreduce=ar)
             ev += r["num_evaluations"]
             cm += r["num_evaluations_computed"]
             bt += r["num_batches"]
             y = r["y"]
-        return {"evals": ev, "computed": cm, "batches": bt, "result": y, "iterations": r["num_iterations"]}
+            for k, v in (("T_camera_lidar", T), ("nm_x", r["x"]), ("nm_cost", r["y"]), ("nm_iterations", r["num_iterations"])):
+                out[k].append(v)
+        return {"evals": ev, "computed": cm, "batches": bt, "result": y, "iterations": r["num_iterations"], "outputs": out}
 
     def e2e_step():
         if grid_mode:
@@ -563,6 +571,8 @@ def main():
         sampler.start()
     res, total_ms, wall, prof = timed(resident_step, args.steps, args.warmup, profile=True)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res[-1]["outputs"])
 
     evals_ref = sum(r["evals"] for r in res)      # what the serial reference would evaluate (this rank's bag / pose share)
     evals_cmp = sum(r["computed"] for r in res)   # poses actually scored
@@ -572,7 +582,7 @@ def main():
     mpoints = world * n_resident * evals_cmp / secs * 1e-6
 
     # ---- e2e: host buffers in, result out, every step -----------------------------------------------------------------------
-    e2e_res, e2e_ms, _, _ = timed(e2e_step, max(3, min(args.steps, 5)), 3, profile=False)
+    e2e_res, e2e_ms, _, _ = timed(e2e_step, args.steps, args.warmup, profile=False)
     e2e_steps = len(e2e_res)
     e2e_evals = sum(r["evals"] for r in e2e_res)
     e2e_cmp = sum(r["computed"] for r in e2e_res)
@@ -617,11 +627,9 @@ def main():
     passes = max(1, prof["passes"])
     t_pass = prof["kernel_ms_total"] * 1e-3 / passes
     achieved = alg_bytes / t_pass * 1e-9
-    ncu = committed_ncu(args.config)
     poses_per_pass = prof["poses_total"] / passes
     roofline = {
         "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-        "traffic": (ncu or {}).get("dram_bytes_per_pass"), "traffic_source": (ncu or {}).get("source"),
         "peak_source": peak_src, "kernel": "nid_persistent_kernel", "us_per_pass": 1e6 * t_pass, "passes_per_launch": passes / max(1, prof["kernel_launches"]),
         "avg_launch_us": 1e3 * prof["kernel_ms_total"] / max(1, prof["kernel_launches"]), "algorithmic_bytes_per_pass": alg_bytes,
         "poses_per_pass": poses_per_pass, "kernel_share_of_step": prof["kernel_ms_total"] / total_ms,
@@ -632,17 +640,9 @@ def main():
         a1 = alg_bytes / (p1["us_per_pass"] * 1e-6) * 1e-9
         roofline["p1"] = {"achieved": a1, "frac": a1 / peak, "us_per_pass": p1["us_per_pass"], "poses_per_pass": 1, "mpoints_per_s": n_resident / p1["us_per_pass"],
                           "note": "same kernel, pose-list mode with one pose per pass (vlcal_nid_set_poses_per_pass): the HBM-bound regime of the path"}
-    # the bound that is active at Nelder-Mead batch sizes: instruction issue.  Instructions per point-pose come from the committed
-    # ncu capture of this config (not hard-coded); 148 SMs x 4 schedulers x 1 warp-instruction/clk x 32 lanes at the sampled clock.
-    sm_clock_hz = 1e6 * (clocks["sm_mhz"] if clocks and clocks.get("sm_mhz") else 1965.0)
-    pp_per_s = n_resident * poses_per_pass / t_pass
-    ipp = (ncu or {}).get("warp_inst_per_pointpose")
-    if ipp:
-        alu_peak = 148 * 4 * 32 * sm_clock_hz / ipp
-        roofline["issue_bound"] = {"achieved_pointposes_per_s": pp_per_s, "peak_pointposes_per_s": alu_peak, "frac": pp_per_s / alu_peak, "warp_inst_per_pointpose": ipp,
-                                   "source": (ncu or {}).get("source")}
-    else:
-        roofline["issue_bound"] = {"achieved_pointposes_per_s": pp_per_s, "warp_inst_per_pointpose": None, "note": "no committed ncu capture for this config"}
+    # the bound that is active at Nelder-Mead batch sizes is instruction issue; its peak needs the executed instructions per
+    # point-pose, which only a profiler capture gives, so only the achieved rate is reported
+    roofline["issue_bound"] = {"achieved_pointposes_per_s": n_resident * poses_per_pass / t_pass}
 
     cpu = None
     if not args.no_cpu_baseline and world == 1:

@@ -1,6 +1,6 @@
-"""B200-native NID LiDAR-camera registration engine (hot path of koide3/direct_visual_lidar_calibration).
+"""GPU-native (H100) NID LiDAR-camera registration engine (hot path of koide3/direct_visual_lidar_calibration).
 
-The compute lives in ``libvlcal_nid.so`` (hand-written sm_100a CUDA behind the C ABI of ``include/vlcal_nid.h``);
+The compute lives in ``libvlcal_nid.so`` (hand-written sm_90a CUDA behind the C ABI of ``include/vlcal_nid.h``);
 this package is the thin host-side mirror of the reference's interface for that path:
 
   create_camera                 <- camera::create_camera             (src/camera/create_camera.cpp:34-50)

@@ -35,7 +35,7 @@ def library_path() -> str:
 
 
 def build_library(force: bool = False, jobs: int = 4) -> str:
-    """Compile libvlcal_nid.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+    """Compile libvlcal_nid.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
     if force:
         subprocess.run(["make", "-C", _CSRC, "clean"], check=True, stdout=subprocess.DEVNULL)
     subprocess.run(["make", "-C", _CSRC, f"-j{jobs}", "-s"], check=True)

@@ -1,7 +1,7 @@
 // lean_filter.cuh -- second-generation fp32 filter of the NID hot loop (reference decisions:
 // src/vlcal/calib/cost_calculator_nid.cpp:31-38): same contract as classify_fast (nid_kernels.cuh) -- a verdict is
 // final only when it is provably the reference's, everything else is re-decided by the exact fp64 path -- but written
-// for instruction count (round-1 profile: 163 warp-instructions per point-pose, 38 % of them arithmetic):
+// for instruction count:
 //
 //   * rounding by the magic constant M = 1.5 * 2^23: t = u' + M holds rint(u') in its low mantissa bits for
 //     |u'| < 2^22, so the pixel index, the distance to the pixel edge and the image-bounds test all come out of two

@@ -1,12 +1,10 @@
-// lean_filter2.cuh -- the lean classifier (lean_filter.cuh) for TWO points at a time on Blackwell's packed fp32 pipe.
+// lean_filter2.cuh -- the lean classifier (lean_filter.cuh) for TWO points at a time.
 //
-// The persistent kernel is bound by instruction issue (profiles/r02_d_*: 76 % of the issue slots, FMA pipe 36 %, ALU pipe
-// 39 %), and about 60 % of what it issues per point-pose are fp32 FMA / MUL / ADD of straight-line chains (rigid transform,
-// distortion polynomial, error-bound polynomials, magic-constant rounding).  sm_100 has FFMA2 / FMUL2 / FADD2
-// (PTX fma/mul/add.rn.f32x2): one instruction, two independent IEEE fp32 operations on a 64-bit register pair, with a
-// scalar-broadcast operand form for the pose entries and camera constants.  A lane already owns K = 2 points of its tile,
-// so the two points ride in the two halves and the fp chains cost half the issue slots; comparisons, selects, MUFU and the
-// integer tail stay scalar per half.
+// The persistent kernel is bound by instruction issue, and most of what it issues per point-pose are fp32 FMA / MUL / ADD
+// of straight-line chains (rigid transform, distortion polynomial, error-bound polynomials, magic-constant rounding).  A
+// lane already owns K = 2 points of its tile, so the two points ride in the two halves of an F2 and their chains are
+// issued interleaved (two independent dependency chains per lane); comparisons, selects, MUFU and the integer tail stay
+// scalar per half.
 //
 // Each half performs exactly the operation sequence of classify_lean (same order, same constants, each result rounded once
 // or -- where the assembler contracts a product into the following sum -- not at all), so the error bounds of
@@ -19,31 +17,17 @@
 namespace vlcal {
 
 struct F2 {
-  unsigned long long v;
+  float lo, hi;
 };
 
-__device__ __forceinline__ F2 f2_pack(float lo, float hi) {
-  F2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "f"(lo), "f"(hi));
-  return r;
-}
+__device__ __forceinline__ F2 f2_pack(float lo, float hi) { return F2{lo, hi}; }
 __device__ __forceinline__ F2 f2_dup(float a) { return f2_pack(a, a); }
-__device__ __forceinline__ void f2_unpack(F2 a, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(a.v)); }
-__device__ __forceinline__ F2 f2_fma(F2 a, F2 b, F2 c) {
-  F2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d.v) : "l"(a.v), "l"(b.v), "l"(c.v));
-  return d;
-}
-__device__ __forceinline__ F2 f2_mul(F2 a, F2 b) {
-  F2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d.v) : "l"(a.v), "l"(b.v));
-  return d;
-}
-__device__ __forceinline__ F2 f2_add(F2 a, F2 b) {
-  F2 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d.v) : "l"(a.v), "l"(b.v));
-  return d;
-}
+__device__ __forceinline__ void f2_unpack(F2 a, float& lo, float& hi) { lo = a.lo, hi = a.hi; }
+// Hopper has no packed fp32 pipe: each half is one FFMA / FMUL / FADD.  The _rn intrinsics are never contracted or
+// reassociated, so every half rounds exactly once, as fma/mul/add.rn.f32x2 would, and the two chains interleave for ILP.
+__device__ __forceinline__ F2 f2_fma(F2 a, F2 b, F2 c) { return F2{__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)}; }
+__device__ __forceinline__ F2 f2_mul(F2 a, F2 b) { return F2{__fmul_rn(a.lo, b.lo), __fmul_rn(a.hi, b.hi)}; }
+__device__ __forceinline__ F2 f2_add(F2 a, F2 b) { return F2{__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)}; }
 __device__ __forceinline__ F2 f2_fma(float a, F2 b, F2 c) { return f2_fma(f2_dup(a), b, c); }
 __device__ __forceinline__ F2 f2_fma(F2 a, F2 b, float c) { return f2_fma(a, b, f2_dup(c)); }
 __device__ __forceinline__ F2 f2_fma(float a, F2 b, float c) { return f2_fma(f2_dup(a), b, f2_dup(c)); }

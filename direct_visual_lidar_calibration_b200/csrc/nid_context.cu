@@ -181,7 +181,7 @@ struct StageLease {
 };
 
 // threads of the copy-convert team.  NOT omp_get_max_threads(): launchers such as torch.distributed.run export
-// OMP_NUM_THREADS=1 for every rank, which silently made the upload serial (6 ms instead of 0.8 ms per 1 M points).
+// OMP_NUM_THREADS=1 for every rank, which silently made the upload serial.
 // The loop is memory-bound: a dozen threads saturate it, waking every core of a 128-core host costs more than it saves.
 static int conversion_threads() {
   static const int n = [] {
@@ -318,8 +318,8 @@ static std::mutex g_geom_mu;
 static std::map<std::tuple<int, const void*, size_t>, int> g_occupancy_cache;
 
 static int hist_copies_cap() {
-  // warp-private copies buy nothing measurable over a couple of shared ones (profiles/r01_microbench.log: 1.32 vs 1.35 T
-  // atomics/s) but every copy is zeroed and merged by every block on every launch; VLCAL_HIST_COPIES overrides for A/B
+  // warp-private copies bought nothing measurable over a couple of shared ones in a shared-atomic microbenchmark
+  // (tools/microbench.cu), but every copy is zeroed and merged by every block on every launch; VLCAL_HIST_COPIES overrides for A/B
   static const int cap = [] {
     const char* e = std::getenv("VLCAL_HIST_COPIES");
     const int v = e ? std::atoi(e) : 2;
@@ -514,11 +514,11 @@ static void fill_common_args(vlcal_nid_ctx* ctx, NidArgs& a) {
 static NidKernel select_kernel(vlcal_nid_ctx* ctx, bool devloop = false) {
   // the fp32 filter needs the float4 layout, a camera/FoV it has bounds for, and 32-bit point indices
   const bool use_filter = ctx->variant != 1 && ctx->cloud->f32 && ctx->fast.enabled && ctx->cloud->n < 0x7fffffffLL;
-  // points per lane and tile (profiles/r01_final_configs.jsonl, r01_final_kernel_scaling.jsonl):
-  //  * fisheye / equirectangular / atan carry transcendental calls and more live state per point: 2 is 2-17 % faster
-  //  * plumb_bob / rational_polynomial / omnidir: 4 wins (6-9 %) while a warp's share of the cloud is a few 128-point
-  //    tiles; below one tile the 4-point path degenerates to single rows, and on long ranges (5 M points) the lighter
-  //    register footprint of 2 wins again (2-5 %)
+  // points per lane and tile (tools/kernel_scaling.py measures the choice):
+  //  * fisheye / equirectangular / atan carry transcendental calls and more live state per point: 2 points
+  //  * plumb_bob / rational_polynomial / omnidir: 4 while a warp's share of the cloud is a few 128-point tiles; below one
+  //    tile the 4-point path degenerates to single rows, and on long ranges (5 M points) the lighter register footprint
+  //    of 2 wins again
   const bool heavy = ctx->cam.model == CAM_FISHEYE || ctx->cam.model == CAM_EQUIRECTANGULAR || ctx->cam.model == CAM_ATAN;
   const long long points_per_warp = ctx->cloud->n / (static_cast<long long>(ctx->num_sms) * 2 * (NID_THREADS / 32));
   const bool four = !heavy && points_per_warp >= 96 && points_per_warp <= 1100;
@@ -539,7 +539,7 @@ static int launch_one(vlcal_nid_ctx* ctx, NidKernel kernel, NidArgs& a, int geom
   const long long want_blocks = (a.n + NID_THREADS - 1) / NID_THREADS;
   const int grid = static_cast<int>(std::max<long long>(1, std::min<long long>(want_blocks, static_cast<long long>(ctx->num_sms) * g.blocks_per_sm)));
   ProfileEvents* ev = nullptr;
-  // event pairs cost ~3 us of host time per launch on the Nelder-Mead critical path: sample one launch in four
+  // event pairs cost host time per launch on the Nelder-Mead critical path: sample one launch in four
   if (ctx->profiling && (ctx->launch_counter++ % PROFILE_STRIDE) == 0) {
     if (ctx->events_used == ctx->events.size()) {
       ProfileEvents e;

@@ -106,7 +106,7 @@ struct vlcal_nid_ctx {
   unsigned long long seq = 0;
   // launch geometry
   int max_poses = 1;
-  int num_sms = 148;
+  int num_sms = 132;  // read from the device at create
   // async state
   bool in_flight = false;
   int in_flight_poses = 0;

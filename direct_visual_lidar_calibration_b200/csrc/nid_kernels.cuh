@@ -1,4 +1,4 @@
-// nid_kernels.cuh -- K1: batched NID joint-histogram kernel with fused finalize (sm_100a).
+// nid_kernels.cuh -- K1: batched NID joint-histogram kernel with fused finalize (sm_90a).
 //
 // Replaces the serial loop of CostCalculatorNID::calculate (reference:
 // src/vlcal/calib/cost_calculator_nid.cpp:30-52) and its entropy/NID tail (:54-64) for P candidate
@@ -47,7 +47,7 @@ struct P2PMailbox {
 // parameters, and the finalizing block -- once the scores of the batch are known -- advances the Nelder-Mead state
 // machine (nm_machine.cuh) and writes the NEXT batch of poses T = init_T * Expmap(x) back into it.  The host can then
 // enqueue many launches back to back without waiting for any of them: the per-iteration host round trip (launch
-// latency + PCIe + wake-up, ~10 us of a ~40 us iteration) disappears from the critical path.  Launches enqueued after
+// latency + PCIe + wake-up) disappears from the critical path.  Launches enqueued after
 // the solver finished see n_poses == 0 and exit at once.
 struct NmDevice {
   NmMachine nm;
@@ -212,7 +212,7 @@ constexpr int FIN_CH = 8;
 
 // natural logarithm for normal, positive, finite arguments (here p + 1e-6 in [1e-6, 1 + 1e-6]), without the special-case
 // branches of the library routine, so that the independent terms a lane evaluates interleave instead of serialising
-// (the library log cost 0.5 us per term in the launch's serial tail).  Algorithm of fdlibm's __ieee754_log (argument
+// (the library log serialised the terms in the launch's serial tail).  Algorithm of fdlibm's __ieee754_log (argument
 // reduction to [sqrt(1/2), sqrt(2)), s = f/(2+f), degree-14 even/odd polynomial split, hi/lo ln2), error < 1 ulp.
 // Every operation is an explicit round-to-nearest intrinsic: the value is a function of x alone, whatever code the call is
 // inlined into (the finalizers of the round-1 kernels and of the persistent kernel must produce the same bits -- the solver

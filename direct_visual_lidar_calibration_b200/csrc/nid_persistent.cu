@@ -41,7 +41,7 @@ static PkKernel pk_pick_ka(int k, int atom) {
 static int pk_tma_requested() {
   static const int v = [] {
     const char* e = std::getenv("VLCAL_PK_TMA");
-    return e ? std::atoi(e) : 0;  // A/B on B200 (profiles/): the staged window does not pay for its index arithmetic -> off
+    return e ? std::atoi(e) : 0;  // A/B: the staged window did not pay for its index arithmetic -> off
   }();
   return v;
 }

@@ -1,15 +1,15 @@
-// nid_persistent.cuh -- K1p: the NID hot path as ONE persistent cooperative kernel per inner solve (sm_100a).
+// nid_persistent.cuh -- K1p: the NID hot path as ONE persistent cooperative kernel per inner solve (sm_90a).
 //
 // Replaces, for a whole dfo::NelderMead<6> inner solve (reference: include/dfo/nelder_mead.hpp:32-101 driving
 // CostCalculatorNID::calculate, src/vlcal/calib/cost_calculator_nid.cpp:21-67, through the objective of
 // src/vlcal/calib/visual_camera_calibration.cpp:103-119), the round-1 scheme "one launch per Nelder-Mead batch + host
-// round trip" (36 us kernel of which ~16 us were launch ramp / serial tail, + ~5 us host gap, x 115 batches at C2).
+// round trip" (a launch ramp, a serial tail and a host gap for every one of the ~115 batches of a C2 solve).
 //
 // One launch, grid = one 768-thread block per SM, all co-resident (cooperative launch, so the waits below cannot deadlock);
 // tile k (64 consecutive points of the tile-ordered cloud) belongs to warp k mod W of its bag for the whole solve.
 // Per Nelder-Mead batch:
 //   (A) every block scores the batch's P <= 8 candidate poses on its tiles -- lean fp32 filter, two points per packed
-//       FFMA2 / FMUL2 / FADD2 (lean_filter.cuh, lean_filter2.cuh), with the exact fp64 recheck for the ~2-3 % of point-poses
+//       two interleaved points per lane (lean_filter.cuh, lean_filter2.cuh), with the exact fp64 recheck for the ~2-3 % of point-poses
 //       near a decision edge (exact_classify.cuh), privatised shared-memory histograms -- and merges its non-zero bins,
 //       its marginals and its inlier counts into the global accumulators (red.global), then arrives (one fence per block);
 //   (B) EVERY block waits for the arrivals and reduces every (bag, pose) accumulator to its NID score itself (:54-64; all
@@ -40,9 +40,9 @@
 namespace vlcal {
 
 // Launch shape: ONE block of 768 threads per SM (24 warps, <= 85 registers).  Three blocks of 256 threads (A/B build,
-// `make alt ALTFLAGS="-DPK_THREADS_CFG=256 -DPK_MIN_BLOCKS=3"`) hold the same 24 warps, but the warp scheduler prefers higher warp slots, so the three blocks of an SM finished
-// their slices at 11 / 14 / 18 us (C2) and every Nelder-Mead batch waited for the 18; one block finishes at 15-16.5 us,
-// merges once instead of three times and arrives once (measured: 28.3 vs 30.8 us per C2 batch, 128 vs 138 us at C3).
+// `make alt ALTFLAGS="-DPK_THREADS_CFG=256 -DPK_MIN_BLOCKS=3"`) hold the same 24 warps, but the warp scheduler prefers higher warp slots, so the three blocks of an SM
+// finish their equal slices at different times and every Nelder-Mead batch waits for the slowest; one block also merges
+// once instead of three times and arrives once.
 #ifndef PK_THREADS_CFG
 #define PK_THREADS_CFG 768
 #endif
@@ -64,7 +64,7 @@ struct alignas(64) PkTensorMap {         // a CUtensorMap (cuTensorMapEncodeTile
   unsigned long long opaque[16];
 };
 #ifndef PK_PACKED_FP32
-#define PK_PACKED_FP32 1  // classify two points per FFMA2 / FMUL2 / FADD2 (lean_filter2.cuh); 0: scalar classifier (A/B build)
+#define PK_PACKED_FP32 1  // classify two points per lane, interleaved (lean_filter2.cuh); 0: scalar classifier (A/B build)
 #endif
 #ifndef PK_DIAG_STAMPS
 #define PK_DIAG_STAMPS 0  // diagnostic build: stamp 3 moves behind the two-ahead zeroing, stamp 5 to the finalizer's inner barrier
@@ -174,7 +174,7 @@ __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int* p) {
   return v;
 }
 
-// histogram increment, two forms (A/B measured on B200, profiles/):
+// histogram increment, two forms (A/B, VLCAL_PK_ATOM):
 //   ATOM == 0: `if (counted) atomicAdd(p, 1)` -- ptxas emits BSSY / BRA / ATOMS.POPC.INC / BSYNC (lanes of a warp that hit
 //              the same bin are merged by the hardware; predication is not available for this form, hence the branch);
 //   ATOM == 1: unconditional red.shared.add of a 0 / 1 register -- one ATOMS.ADD, no branch, same-bin lanes serialise.
@@ -450,7 +450,7 @@ static __device__ __noinline__ void nm_warp_step(NmMachine& s, const double* ys,
 // T = init_T * Expmap(x) (visual_camera_calibration.cpp:104) for the n_cand <= 8 pending candidates, by one warp: lane 3c + i
 // computes row i of candidate c.  Same operations in the same order as se3_expmap_gtsam_hd + isometry_mul_hd (se3_math.cuh)
 // for every matrix entry (the rows of R, t and of the product are independent of each other), so the poses are
-// bit-identical to the serial code; the serial version cost ~3 us of every Nelder-Mead batch on one lane.
+// bit-identical to the serial code, which ran on one lane in every Nelder-Mead batch.
 static __device__ __noinline__ void pk_poses_of_candidates(PkShared& sh, int n_cand, int lane) {
   const int c = lane / 3, i = lane - 3 * c;
   const bool active = c < n_cand;
@@ -871,9 +871,8 @@ __device__ __forceinline__ void pk_tile(const PkArgs& a, const PkShared& sh, con
     }
   }
   // Deferred (point, pose) pairs of this tile -> the warp's queue for the exact path.  Doing this once per tile instead of inside the pose loop
-  // matters: with ~3 % of the point-poses deferred, SOME lane of the 32 x K has one in 5 of 6 pose steps, and the ballot /
-  // queue code (~95 instructions) ran almost every step -- 160 executed instructions per point-pose against 109 in the
-  // straight-line path (profiles/r02_c_*).
+  // matters: with ~3 % of the point-poses deferred, SOME lane of the 32 x K has one in 5 of 6 pose steps, so the ballot /
+  // queue code would run almost every step instead of once per tile.
   // Usual case (the tile defers at most 32 pairs): one warp prefix sum gives every lane the queue slots of its pairs.
   // Otherwise: one ballot per round.
   const int cnt = __popc(unc_mask);
@@ -1147,10 +1146,9 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
       // Interleaved split: tile k (32 * K consecutive points of the tile-ordered cloud) goes to warp k mod W of the bag, so
       // every warp -- and every block: its 24 warps take 24 neighbouring tiles per round -- samples the whole image instead of
       // owning one region.  With contiguous slices the cost of a slice followed its region (deferred rechecks, histogram bin
-      // collisions, cache hit rates): the slowest block finished 35 % (C2) / 14 % (C3) after the median one, and every
-      // Nelder-Mead batch waits for the slowest.  (Claiming tiles from an atomic counter was measured too: no better than
-      // the contiguous split at 256-point claims -- one claim is ~20 us of work for a warp -- and finer claims serialise on
-      // the counter.)  The next tile's rows are in flight while the current one is swept over the poses.
+      // collisions, cache hit rates), so the slowest block finished well after the median one, and every Nelder-Mead batch
+      // waits for the slowest.  (Claiming tiles from an atomic counter was tried too: no better than the contiguous split
+      // at 256-point claims, and finer claims serialise on the counter.)  The next tile's rows are in flight while the current one is swept over the poses.
       constexpr unsigned int TP = 32u * K;
       unsigned int tile = warp_global;
       float4 qk[K];
@@ -1259,8 +1257,7 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
     }
     // ---- (B, Nelder-Mead) every block finalizes every (bag, pose) of the batch itself, one warp per item ---------------------
     // The next step of the solve needs all scores in every block.  An owner block per item (round-2 first version) cost a
-    // second hop -- all arrived -> owner computes with the whole block -> fence -> publishes -> everybody polls: 4.4 us of
-    // the 26 us batch at C2 -- and the zero-on-read accumulator needed that fence.  Here the arrival wait is the only hop:
+    // second hop -- all arrived -> owner computes with the whole block -> fence -> publishes -> everybody polls -- and the zero-on-read accumulator needed that fence.  Here the arrival wait is the only hop:
     // each block reads the merged accumulators (4 KB per item, L2) and computes the same canonical NID per item in one warp.
     // Accumulators rotate over three buffers and are zeroed two batches ahead: buffer (batch + 2) % 3 was last read in
     // batch - 1 (finished by every block before it arrived here) and is next merged in batch + 2, which no block reaches

@@ -1,5 +1,5 @@
 // nid_cost_cuda.hpp -- reference-side binding for the NID_BFGS branch: keeps Ceres and the Sophus manifold, replaces
-// the per-bag cost functor and its autodiff by the sm_100a value + gradient kernel of libvlcal_nid.so.
+// the per-bag cost functor and its autodiff by the sm_90a value + gradient kernel of libvlcal_nid.so.
 //
 // In VisualCameraCalibration::estimate_pose_bfgs (src/vlcal/calib/visual_camera_calibration.cpp:187-238) the reference
 // builds, per bag,   std::shared_ptr<NIDCost>(new NIDCost(proj, normalized_image, culled_points, bins))        (:203)

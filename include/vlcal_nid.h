@@ -1,5 +1,5 @@
 /*
- * vlcal_nid.h -- C ABI of the B200-native NID registration engine (libvlcal_nid.so).
+ * vlcal_nid.h -- C ABI of the GPU-native (H100) NID registration engine (libvlcal_nid.so).
  *
  * This is the drop-in boundary for ONE hot path of koide3/direct_visual_lidar_calibration:
  * the per-evaluation NID cost and the Nelder-Mead solve that drives it.  Every entry point
@@ -270,9 +270,9 @@ int vlcal_generate_lidar_image(
  *   1 host loop: one launch per Nelder-Mead batch, scores published to mapped host memory, host polls.
  *   2 device-resident loop (one local bag; scores local or summed by the in-kernel peer exchange): the state machine
  *     advances inside the kernel's finalizing block, launches are enqueued back to back; VLCAL_ERR_UNSUPPORTED otherwise.
- * Both loops run the same state machine (bit-identical trajectory, tests/test_gpu_parity.py).  Measured on B200 at the C2
- * size the host loop is the faster one (38 vs 48 us per batch: stepping the machine + Expmap on one SM costs more than the
- * host round trip it removes), hence the default; with mode 2 params.callback is delivered from the evaluation trace, in
+ * Both loops run the same state machine (bit-identical trajectory, tests/test_gpu_parity.py).  At the C2 size the host
+ * loop was measured the faster one (stepping the machine + Expmap on one SM costs more than the host round trip it
+ * removes), hence the default; with mode 2 params.callback is delivered from the evaluation trace, in
  * the reference's order, up to one chunk of launches late. */
 int vlcal_nid_set_solver_mode(int mode);
 

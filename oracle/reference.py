@@ -1,8 +1,10 @@
-"""ctypes binding of oracle/_ref/libvlcal_ref.so -- the REFERENCE's own sources of the NID path, compiled from
-/root/reference against the stand-in headers in oracle/ref_standin/ (oracle/ref_shim.cpp, `make -C oracle ref`).
+"""ctypes binding of oracle/_ref/libvlcal_ref.so -- the REFERENCE's own sources of the NID path, compiled from a
+reference checkout against the stand-in headers in oracle/ref_standin/ (oracle/ref_shim.cpp,
+`make -C oracle ref REF=<checkout>`, or build() with VLCAL_REFERENCE=<checkout> in the environment).
 
-TEST INFRASTRUCTURE ONLY: it exists to pin oracle/vlcal_oracle.c (tests/test_reference_pin.py).  The library is
-git-ignored; it is built in the container that has /root/reference and travels to the GPU box as a built file.
+TEST INFRASTRUCTURE ONLY: tests/golden/make_reference_outputs.py uses it to record what the reference returns on the test
+inputs (tests/golden/reference_outputs.json), which tests/test_reference_pin.py pins the oracle against.  The library is
+git-ignored.
 """
 from __future__ import annotations
 
@@ -14,7 +16,7 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_ref", "libvlcal_ref.so")
-REFERENCE_ROOT = "/root/reference"
+REFERENCE_ROOT = os.environ.get("VLCAL_REFERENCE", "")  # a checkout of koide3/direct_visual_lidar_calibration
 
 NM_FUNC = C.CFUNCTYPE(C.c_double, C.POINTER(C.c_double), C.c_void_p)
 _lib = None
@@ -23,8 +25,8 @@ _lib = None
 def build() -> str | None:
     """(Re)build when the reference tree is present; returns the library path, or None when there is neither a
     reference tree nor a prebuilt library."""
-    if os.path.isdir(os.path.join(REFERENCE_ROOT, "src")):
-        subprocess.run(["make", "-C", _HERE, "-s", "ref"], check=True)
+    if REFERENCE_ROOT and os.path.isdir(os.path.join(REFERENCE_ROOT, "src")):
+        subprocess.run(["make", "-C", _HERE, "-s", "ref", f"REF={REFERENCE_ROOT}"], check=True)
     return LIB_PATH if os.path.exists(LIB_PATH) else None
 
 

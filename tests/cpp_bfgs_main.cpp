@@ -1,39 +1,27 @@
-// Compiles include/vlcal_b200/nid_cost_cuda.hpp and cost_calculator_nid_cuda.hpp against the REFERENCE's own headers
-// (include/vlcal/..., include/camera/...) plus the stand-in third-party headers of oracle/ref_standin, and drives
+// Compiles include/vlcal_b200/nid_cost_cuda.hpp (the NID_BFGS binding) against the stand-in third-party headers of
+// oracle/ref_standin (Ceres, Sophus, Eigen, cv::Mat) and the Frame stand-in of tests/cpp_stubs, and drives
 // MultiNIDCostFunction the way visual_camera_calibration.cpp:208-228 would: through ceres::FirstOrderFunction.
+// Output: "EVAL ok=<0|1> n=<parameters> cost=<value> g0=<d cost / d qx>", or "EXCEPTION <message>" with exit code 3.
 #include <cstdio>
 #include <memory>
 #include <vector>
 
-#include <vlcal_b200/cost_calculator_nid_cuda.hpp>
 #include <vlcal_b200/nid_cost_cuda.hpp>
-
-namespace vlcal {  // members whose reference translation units (frame_cpu.cpp, visual_lidar_data.cpp) are not compiled here
-FrameCPU::FrameCPU() {}
-FrameCPU::~FrameCPU() {}
-VisualLiDARData::~VisualLiDARData() {}
-NIDCostParams::NIDCostParams() { bins = 16; }  // src/vlcal/calib/cost_calculator_nid.cpp:7-9
-NIDCostParams::~NIDCostParams() {}
-}  // namespace vlcal
 
 int main() {
   const int W = 64, H = 48, N = 500;
-  std::vector<unsigned char> pixels(W * H, 100);
-  std::vector<Eigen::Vector4d> pts(N, Eigen::Vector4d(0.1, 0.05, 2.0, 1.0));
-  std::vector<double> intens(N, 0.5);
-  auto frame = std::make_shared<vlcal::FrameCPU>();
+  std::vector<unsigned char> pixels(W * H);
+  for (int i = 0; i < W * H; i++) pixels[i] = static_cast<unsigned char>((i * 37) % 251);
+  std::vector<Eigen::Vector4d> pts;
+  std::vector<double> intens;
+  for (int i = 0; i < N; i++) {  // a patch in front of the camera (z = 2 m), spread over most of the image
+    pts.emplace_back(-0.8 + 1.6 * (i % 25) / 24.0, -0.6 + 1.2 * (i / 25) / 19.0, 2.0, 1.0);
+    intens.push_back((i % 16) / 16.0);
+  }
+  auto frame = std::make_shared<vlcal::Frame>();
   frame->num_points = N, frame->points = pts.data(), frame->intensities = intens.data();
   const cv::Mat image(H, W, CV_8UC1, pixels.data(), static_cast<size_t>(W));
   try {
-    {  // the reference's own factory behind the parameter view: CostCalculatorNIDCuda(proj, data, params)
-      const auto proj = vlcal::create_camera_with_params("plumb_bob", std::vector<double>{60.0, 60.0, 32.0, 24.0}, std::vector<double>{});
-      auto data = std::make_shared<vlcal::VisualLiDARData>();
-      data->image = image;
-      data->points = frame;
-      const Eigen::Vector2d uv = proj->project(Eigen::Vector3d(0.1, 0.05, 2.0));  // forwarded to the reference's PinholeProjection
-      std::shared_ptr<vlcal::CostCalculator> cost = std::make_shared<vlcal::CostCalculatorNIDCuda>(proj, data, vlcal::NIDCostParams());
-      std::printf("VIEW u=%.6f nid=%.17g\n", uv[0], cost->calculate(Eigen::Isometry3d::Identity()));
-    }
     const Sophus::SE3d init;
     auto* fn = new vlcal::MultiNIDCostFunction(init);
     fn->add(std::make_shared<vlcal::NIDCostCuda>("plumb_bob", std::vector<double>{60.0, 60.0, 32.0, 24.0}, std::vector<double>{}, image, frame, 16));

@@ -1,5 +1,6 @@
-"""The reference-side C++ binding (include/vlcal_b200/cost_calculator_nid_cuda.hpp) compiles against stand-in
-reference headers, links to the C-ABI library, and behaves like a vlcal::CostCalculator."""
+"""The reference-side C++ bindings compile against stand-in reference headers and link to the C-ABI library:
+include/vlcal_b200/cost_calculator_nid_cuda.hpp behaves like a vlcal::CostCalculator, and
+include/vlcal_b200/nid_cost_cuda.hpp (the NID_BFGS branch) like the ceres::FirstOrderFunction it replaces."""
 import os
 import struct
 import subprocess
@@ -59,20 +60,43 @@ def test_shim_matches_python_surface_and_oracle(gpu, oracle, tmp_path):
     assert abs(vals[0] - onid) < 1e-12
 
 
-REFERENCE = "/root/reference"
-
-
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REFERENCE, "include")), reason="needs the reference tree's headers (this container only)")
-def test_bindings_compile_inside_the_reference_tree(vlcal, tmp_path):
-    """Both reference-side bindings against the reference's OWN headers (third-party ones from oracle/ref_standin):
-    cost_calculator_nid_cuda.hpp (Nelder-Mead branch) and nid_cost_cuda.hpp (BFGS branch, a ceres::FirstOrderFunction)."""
+def _build_bfgs(vlcal, tmp_path):
+    """tests/cpp_bfgs_main.cpp: the BFGS binding against the Ceres / Sophus / Eigen / cv::Mat stand-ins of oracle/ref_standin
+    (listed first, so they win over tests/cpp_stubs, which only adds vlcal/common/frame.hpp here)."""
     exe = str(tmp_path / "cpp_bfgs")
     libdir = os.path.dirname(vlcal.library_path())
-    cmd = ["/usr/bin/g++", "-std=c++17", "-O1", "-w", "-I", os.path.join(ROOT, "oracle", "ref_standin"), "-I", os.path.join(REFERENCE, "include"), "-I", os.path.join(ROOT, "include"),
-           os.path.join(HERE, "cpp_bfgs_main.cpp"), os.path.join(REFERENCE, "src", "camera", "create_camera.cpp"), "-o", exe, "-L", libdir, "-lvlcal_nid", f"-Wl,-rpath,{libdir}"]
+    cmd = ["/usr/bin/g++", "-std=c++17", "-O1", "-Wall", "-I", os.path.join(ROOT, "oracle", "ref_standin"), "-I", os.path.join(HERE, "cpp_stubs"),
+           "-I", os.path.join(ROOT, "include"), os.path.join(HERE, "cpp_bfgs_main.cpp"), "-o", exe, "-L", libdir, "-lvlcal_nid", f"-Wl,-rpath,{libdir}"]
     subprocess.run(cmd, check=True)
-    out = subprocess.run([exe], capture_output=True, text=True)
+    return exe
+
+
+def test_bfgs_binding_compiles_and_fails_loudly_without_gpu(vlcal, tmp_path):
+    exe = _build_bfgs(vlcal, tmp_path)
     if vlcal.device_count() > 0:
-        assert out.returncode == 0 and out.stdout.startswith("EVAL ok="), out.stdout + out.stderr
-    else:  # no CPU fallback: the constructor throws with the library's message
-        assert out.returncode == 3 and "EXCEPTION" in out.stdout, out.stdout + out.stderr
+        pytest.skip("a GPU is present; covered by the gpu test")
+    out = subprocess.run([exe], capture_output=True, text=True)
+    # no CPU fallback: the NIDCostCuda constructor throws with the library's message
+    assert out.returncode == 3 and out.stdout.startswith("EXCEPTION") and "no CUDA device" in out.stdout, out.stdout + out.stderr
+
+
+def _bfgs_main_problem():
+    """The inputs tests/cpp_bfgs_main.cpp builds: a 64x48 image, 500 points on a plane 2 m in front of the camera."""
+    W, H, N = 64, 48, 500
+    image = ((np.arange(W * H) * 37) % 251).astype(np.uint8).reshape(H, W)
+    i = np.arange(N)
+    pts = np.stack([-0.8 + 1.6 * (i % 25) / 24.0, -0.6 + 1.2 * (i // 25) / 19.0, np.full(N, 2.0), np.ones(N)], axis=1)
+    return image, pts, (i % 16) / 16.0
+
+
+@pytest.mark.gpu
+def test_bfgs_binding_matches_python_surface(gpu, tmp_path):
+    exe = _build_bfgs(gpu, tmp_path)
+    out = subprocess.run([exe], capture_output=True, text=True)
+    assert out.returncode == 0 and out.stdout.startswith("EVAL ok=1 n=7 "), out.stdout + out.stderr
+    fields = dict(kv.split("=") for kv in out.stdout.split()[1:])
+    image, pts, ins = _bfgs_main_problem()
+    cam = gpu.create_camera("plumb_bob", [60.0, 60.0, 32.0, 24.0], [])
+    ok, nid, grad = gpu.NIDCost(cam, gpu.VisualLiDARData(image, pts, ins), 16).evaluate_with_gradient(np.array([[0, 0, 0, 1, 0, 0, 0.0]]))
+    assert bool(ok[0]) and np.isfinite(nid[0])
+    assert abs(float(fields["cost"]) - nid[0]) < 1e-12 and abs(float(fields["g0"]) - grad[0][0]) < 1e-12 * max(1.0, abs(grad[0][0]))

@@ -28,11 +28,11 @@ def test_library_exports_every_declared_symbol(vlcal):
     assert not missing, missing
 
 
-def test_library_has_sm100a_code(vlcal):
+def test_library_has_sm90a_code(vlcal):
     out = subprocess.run(["cuobjdump", "-lelf", vlcal.library_path()], capture_output=True, text=True)
     if out.returncode != 0:
         pytest.skip("cuobjdump unavailable")
-    assert "sm_100a" in out.stdout
+    assert "sm_90a" in out.stdout
 
 
 def test_product_does_not_link_or_import_the_oracle(vlcal):

@@ -1,6 +1,6 @@
-// tools/microbench.cu -- B200 micro-measurements that drive the design of the NID kernel (DESIGN.md cites the
+// tools/microbench.cu -- micro-measurements that drive the design of the NID kernel (DESIGN.md cites the
 // numbers): shared-memory histogram atomics, fp64 vs fp32 issue rates (mul/add, div, sqrt), random 1-byte gathers
-// from an L2-resident image.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/microbench tools/microbench.cu
+// from an L2-resident image.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/microbench tools/microbench.cu
 #include <cuda_runtime.h>
 
 #include <cstdio>

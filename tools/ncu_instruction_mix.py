@@ -2,7 +2,7 @@
 """Executed-instruction breakdown of one persistent-kernel capture from `ncu -i <rep> --page source --csv`:
 per code region (contiguous SASS ranges with similar execution counts) and per opcode, with the stall-sample share.
 
-  ncu -i gpurun_out/<capture>.ncu-rep --page source --csv > /tmp/source.csv
+  ncu -i <capture>.ncu-rep --page source --csv > /tmp/source.csv
   python tools/ncu_instruction_mix.py /tmp/source.csv > profiles/<name>_instruction_mix.txt"""
 import csv
 import sys

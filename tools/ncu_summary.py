@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Summarise one `ncu --set full` capture of the persistent kernel into profiles/r02_ncu_<config>.json -- the figures that
-only a profiler gives and that bench.py reports beside its own CUDA-event timings (never a number measured under ncu as a
-bench value): DRAM traffic per pass over the cloud, executed warp instructions per point-pose, issue utilisation.
+"""Summarise one `ncu --set full` capture of the persistent kernel into profiles/ncu_<config>.json (profiles/ is a local,
+git-ignored directory) -- the figures that only a profiler gives, to be read beside bench.py's CUDA-event timings (never a
+number measured under ncu as a bench value): DRAM traffic per pass over the cloud, executed warp instructions per point-pose, issue utilisation.
 
-  python tools/ncu_summary.py gpurun_out/<capture>.ncu-rep --config C3 --points 4902806 --poses 1055 --passes 261
+  python tools/ncu_summary.py <capture>.ncu-rep --config C3 --points 4902806 --poses 1055 --passes 261
 (points = cloud size of the profiled context, poses / passes = point-pose passes the captured launch carried; the probe
 tools print them)."""
 import argparse
@@ -42,7 +42,7 @@ def main():
     inst = num("smsp__inst_executed.sum")
     dur = num("gpu__time_duration.sum")
     out = {
-        "source": f"profiles/{os.path.basename(args.report).replace('.ncu-rep', '')} (ncu --set full --clock-control none, one launch of {m['Kernel Name'][0] if 'Kernel Name' in m else 'nid_persistent_kernel'})",
+        "source": f"{os.path.basename(args.report)} (ncu --set full --clock-control none, one launch of {m['Kernel Name'][0] if 'Kernel Name' in m else 'nid_persistent_kernel'})",
         "config": args.config, "points": args.points, "poses": args.poses, "passes": args.passes,
         "duration_under_ncu_ms": dur * 1e3,
         "dram_bytes_per_launch": dram, "dram_bytes_per_pass": dram / args.passes,
@@ -55,7 +55,8 @@ def main():
         "stalls_per_issue": {k.split("issue_stalled_")[1].split("_per_issue")[0]: float(v[0]) for k, v in m.items() if k.startswith("smsp__average_warps_issue_stalled_") and k.endswith("_per_issue_active.ratio")},
         "note": args.note or "instruction count includes the spin-waits of the persistent kernel's barriers (thread 0 of every block polls) and the exact fp64 rechecks",
     }
-    path = args.out or os.path.join(ROOT, "profiles", f"r02_ncu_{args.config}.json")
+    path = args.out or os.path.join(ROOT, "profiles", f"ncu_{args.config}.json")
+    os.makedirs(os.path.dirname(path) or ".", exist_ok=True)
     json.dump(out, open(path, "w"), indent=1)
     print(json.dumps(out, indent=1))
 

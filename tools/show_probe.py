@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""Compact view of a tools/pk_probe.py JSON-lines file (or a gpurun log that contains such lines)."""
+"""Compact view of a tools/pk_probe.py JSON-lines file (or a log that contains such lines)."""
 import json
 import sys
 
 for line in open(sys.argv[1]):
     line = line.strip()
     if not line.startswith('{"config"'):
-        if line and not line.startswith(".") and "[gpurun] send" not in line:
+        if line and not line.startswith("."):
             print(line[:300])
         continue
     try:
