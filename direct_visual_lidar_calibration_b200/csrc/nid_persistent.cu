@@ -38,6 +38,12 @@ static PkKernel pk_pick_ka(int k, int atom) {
   return atom ? nid_persistent_kernel<MODEL, 2, 1> : nid_persistent_kernel<MODEL, 2, 0>;
 }
 
+// the points per lane of the kernel pk_pick_ka returns for a requested k
+static int pk_kernel_k(int model, int k) {
+  const bool heavy = model == CAM_FISHEYE || model == CAM_EQUIRECTANGULAR || model == CAM_ATAN;
+  return k == 4 && (!heavy || PK_K4_ALL) ? 4 : 2;
+}
+
 static int pk_tma_requested() {
   static const int v = [] {
     const char* e = std::getenv("VLCAL_PK_TMA");
@@ -102,24 +108,41 @@ static PkKernel pk_pick(int model, int k) {
 struct PkGeom {
   int copies;
   size_t smem;
+  unsigned int ring_off;  // byte offset of the tile rings in dynamic shared memory
   int max_blocks;  // co-resident blocks of the whole device (cooperative launch limit)
 };
 
 static std::mutex g_pk_mu;
 static std::map<std::tuple<int, const void*, size_t>, int> g_pk_occupancy;
 
-static int pk_geometry(int device, int num_sms, PkKernel kernel, int nb, PkGeom* g, bool tma = false) {
+// Dynamic shared memory of one block: the histogram copies (whose space the finalizer reuses as staging), then either
+// the TMA variant's image window or the warps' tile rings.  At 16 bins and K = 2: 48 KB of copies + 24 warps x 2 slots
+// x 1 KB of rings = 96 KB, next to ~16 KB of static PkShared -- within the 227 KB a block may opt in to on an H100.
+static int pk_geometry(int device, int num_sms, PkKernel kernel, int nb, int kpt, PkGeom* g, bool tma = false) {
   // histogram copies for 8 poses (the initial simplex of a 6-D solve is 7) -- two copies while they fit 64 KB
   const size_t per_copy = static_cast<size_t>(PK_MAX_POSES) * nb * sizeof(int);
   g->copies = static_cast<int>(std::max<size_t>(1, std::min<size_t>(PK_WARPS / 4, (64 * 1024) / per_copy)));  // one copy per four warps
   const size_t scratch = static_cast<size_t>(nb) * 8 + 64 * 8 * 2 + 64 * 4 * 2;  // pk_block_nid staging (aliases the copies)
   g->smem = std::max(per_copy * g->copies, scratch);
-  if (tma) g->smem = ((g->smem + 127) & ~static_cast<size_t>(127)) + PK_TMA_BYTES;
+  const size_t tail = (g->smem + 127) & ~static_cast<size_t>(127);
+  g->ring_off = static_cast<unsigned int>(tail);
+  if (tma) g->smem = tail + PK_TMA_BYTES;
+  else if (PK_TILE_RING) g->smem = tail + pk_ring_bytes(kpt);
   std::lock_guard<std::mutex> lock(g_pk_mu);
   const auto key = std::make_tuple(device, reinterpret_cast<const void*>(kernel), g->smem);
   auto it = g_pk_occupancy.find(key);
   if (it == g_pk_occupancy.end()) {
-    VL_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(128 * 1024)));
+    int optin = 0;
+    VL_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+    cudaFuncAttributes fa;
+    VL_CUDA(cudaFuncGetAttributes(&fa, kernel));
+    const size_t dyn_max = static_cast<size_t>(optin) - fa.sharedSizeBytes;
+    if (g->smem > dyn_max) {
+      set_last_error("persistent kernel: " + std::to_string(g->smem) + " bytes of dynamic shared memory exceed the " + std::to_string(dyn_max) + " the device allows");
+      return VLCAL_ERR_UNSUPPORTED;
+    }
+    // the opt-in limit is a property of the kernel: set it to the device's maximum, whatever this launch asks for
+    VL_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn_max)));
     int nblk = 0;
     VL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nblk, kernel, PK_THREADS, g->smem));
     it = g_pk_occupancy.emplace(key, std::max(1, nblk)).first;
@@ -205,6 +228,7 @@ void pk_fill_common(PkArgs& a, vlcal_nid_ctx* const* ctxs, int n_ctxs, const PkG
   a.lean = c0->lean;
   a.n_bags = n_ctxs;
   a.copies = g.copies;
+  a.ring_off = g.ring_off;
   // blocks per bag in proportion to the point counts, at least one each
   long long total_points = 0;
   for (int i = 0; i < n_ctxs; i++) total_points += std::max<long long>(1, ctxs[i]->cloud->n);
@@ -258,7 +282,7 @@ int pk_solve(
   if (use_tma) kernel = pk_pick_tma(c0->cam.model, kpt);
   PkGeom g;
   {
-    const int rc = pk_geometry(c0->device, c0->num_sms, kernel, c0->bins * c0->bins, &g, use_tma);
+    const int rc = pk_geometry(c0->device, c0->num_sms, kernel, c0->bins * c0->bins, pk_kernel_k(c0->cam.model, kpt), &g, use_tma);
     if (rc != VLCAL_OK) return rc;
   }
   const int grid = pk_grid_size(g, ctxs, n_ctxs);
@@ -432,10 +456,11 @@ int pk_score_poses(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_colma
   VL_CUDA(cudaSetDevice(c0->device));
   long long total_points = 0;
   for (int i = 0; i < n_ctxs; i++) total_points += ctxs[i]->cloud->n;
-  PkKernel kernel = pk_pick(c0->cam.model, pk_points_per_lane(c0, total_points));
+  const int kpt = pk_points_per_lane(c0, total_points);
+  PkKernel kernel = pk_pick(c0->cam.model, kpt);
   PkGeom g;
   {
-    const int rc = pk_geometry(c0->device, c0->num_sms, kernel, c0->bins * c0->bins, &g);
+    const int rc = pk_geometry(c0->device, c0->num_sms, kernel, c0->bins * c0->bins, pk_kernel_k(c0->cam.model, kpt), &g);
     if (rc != VLCAL_OK) return rc;
   }
   const int grid = pk_grid_size(g, ctxs, n_ctxs);

@@ -72,6 +72,18 @@ struct alignas(64) PkTensorMap {         // a CUtensorMap (cuTensorMapEncodeTile
 #ifndef PK_MIN_BLOCKS
 #define PK_MIN_BLOCKS 1  // blocks per SM the register allocation must allow (768 threads x 85 registers fill the register file)
 #endif
+// Tile ring (interleaved split, not the TMA variant): every warp streams its tiles through PK_RING_SLOTS shared-memory
+// slots filled by per-lane 16-byte cp.async copies; 0: the next tile's rows are prefetched into registers (A/B build)
+#ifndef PK_TILE_RING
+#define PK_TILE_RING 1
+#endif
+#ifndef PK_RING_SLOTS
+#define PK_RING_SLOTS 2  // PK_RING_SLOTS - 1 tiles in flight; every slot more takes 24 KB of the SM's L1 for shared memory
+#endif
+constexpr int PK_RING = PK_RING_SLOTS;
+static_assert(PK_RING >= 2 && PK_RING <= 8, "PK_RING_SLOTS: 2..8 tile slots per warp");
+// dynamic shared memory of the block's tile rings: PK_WARPS x PK_RING slots of one 32*k-point tile (float4 rows)
+__host__ __device__ constexpr unsigned int pk_ring_bytes(int k) { return PK_TILE_RING ? static_cast<unsigned int>(PK_WARPS * PK_RING * 32 * k * 16) : 0u; }
 
 // score exchange: every double travels as two 8-byte words {32 data bits | 32-bit sequence tag} (an aligned 8-byte store
 // is never torn, so the data is its own arrival flag).  w[slot][(rank * n_bags + bag) * 8 + pose][lo, hi]
@@ -111,6 +123,7 @@ struct PkArgs {
   int n_bags;
   PkBag bag[PK_MAX_BAGS];
   int copies;  // shared-memory histogram copies per block
+  unsigned int ring_off;  // byte offset of the tile rings in dynamic shared memory (128-byte aligned, behind the histogram copies)
   // work source
   const PkSolve* solve;      // Nelder-Mead mode when non-null
   PkResult* result_host;     // Nelder-Mead mode: outcome (mapped pinned host memory)
@@ -164,6 +177,7 @@ struct PkShared {
   unsigned int q_idx[PK_WARPS][PK_QUEUE];
   unsigned char q_pose[PK_WARPS][PK_QUEUE];
   int q_cnt[PK_WARPS];  // fill count of each warp's queue
+  uint4 ring_state[PK_WARPS];  // tile ring bookkeeping of each warp: {next tile, tiles left in the pass, tile step, slot}
 };
 
 // ---- small PTX helpers ---------------------------------------------------------------------------------------------
@@ -765,19 +779,26 @@ struct PkBagRegs {
   const uint8_t* bin_image;
 };
 
+// the call takes the warp's state by value: a reference would force PkWarp into local memory for the whole hot loop
 template <int MODEL>
-__device__ __noinline__ void pk_drain32(const PkArgs& a, const PkShared& sh, const PkBagRegs& B, PkWarp& w, int first, int count) {
-  if (w.lane < count) {  // one deferred (point, pose) per lane, exact path
-    const unsigned int i = lds_u32(w.q_idx + 4u * static_cast<unsigned int>(first + w.lane));
-    const int p = static_cast<int>(lds_u8(w.q_pose + static_cast<unsigned int>(first + w.lane)));
-    const float4 q = __ldg(B.points + i);
+__device__ __noinline__ void pk_drain32_impl(const PkArgs& a, const PkShared& sh, const float4* points, const uint8_t* bin_image, unsigned int hist_addr, unsigned int q_idx, unsigned int q_pose,
+                                             int lane, int first, int count) {
+  if (lane < count) {  // one deferred (point, pose) per lane, exact path
+    const unsigned int i = lds_u32(q_idx + 4u * static_cast<unsigned int>(first + lane));
+    const int p = static_cast<int>(lds_u8(q_pose + static_cast<unsigned int>(first + lane)));
+    const float4 q = __ldg(points + i);
     const int pix = exact_pixel_hd<MODEL>(a.cam, a.cos_fov, a.width, a.height, sh.pose64[p], q.x, q.y, q.z);
     if (pix >= 0) {
-      const int ib = __ldg(B.bin_image + pix);  // :43,:46 via the pre-binned image
-      const unsigned int addr = w.hist_addr + 4u * static_cast<unsigned int>(p * a.nb + ib + lidar_bin_of(q.w, a.bins) * a.bins);
+      const int ib = __ldg(bin_image + pix);  // :43,:46 via the pre-binned image
+      const unsigned int addr = hist_addr + 4u * static_cast<unsigned int>(p * a.nb + ib + lidar_bin_of(q.w, a.bins) * a.bins);
       asm volatile("red.shared.add.u32 [%0], 1;" ::"r"(addr) : "memory");  // :49 hist(image_bin, lidar_bin)++
     }
   }
+}
+
+template <int MODEL>
+__device__ __forceinline__ void pk_drain32(const PkArgs& a, const PkShared& sh, const PkBagRegs& B, const PkWarp& w, int first, int count) {
+  pk_drain32_impl<MODEL>(a, sh, B.points, B.bin_image, w.hist_addr, w.q_idx, w.q_pose, w.lane, first, count);
 }
 
 // one tile = 32*K consecutive points starting at `tile`, swept over the P poses of the batch; the image-bin gathers of
@@ -938,6 +959,21 @@ __device__ __forceinline__ void pk_load_tile(const float4* __restrict__ pts, uns
   }
 }
 
+// points [tpos, end) of the cloud in single-row tiles, the next row in flight
+template <int MODEL, int ATOM, bool TMA>
+__device__ __forceinline__ void pk_rows(const PkArgs& a, const PkShared& sh, const PkBagRegs& B, int n_poses, PkWarp& w, unsigned int tpos, unsigned int end) {
+  const int lane = w.lane;
+  float4 q1[1], n1[1];
+  if (tpos < end) pk_load_tile<1>(B.points, tpos, end, lane, q1);
+  while (tpos < end) {
+    const bool more = tpos + 32u < end;
+    if (more) pk_load_tile<1>(B.points, tpos + 32u, end, lane, n1);
+    pk_tile<MODEL, 1, true, ATOM, TMA>(a, sh, B, n_poses, w, tpos, end, q1);
+    tpos += 32u;
+    if (more) q1[0] = n1[0];
+  }
+}
+
 // points [tpos, end) of the cloud: K-row tiles with the next tile's rows in flight, then single-row tiles for the rest;
 // qk holds the first K-row tile when `first_loaded`
 template <int MODEL, int K, int ATOM, bool TMA>
@@ -955,15 +991,40 @@ __device__ __forceinline__ void pk_range(const PkArgs& a, const PkShared& sh, co
       for (int j = 0; j < K; j++) qk[j] = nxt[j];
     }
   }
-  float4 q1[1], n1[1];
-  if (tpos < end) pk_load_tile<1>(B.points, tpos, end, lane, q1);
-  while (tpos < end) {
-    const bool more = tpos + 32u < end;
-    if (more) pk_load_tile<1>(B.points, tpos + 32u, end, lane, n1);
-    pk_tile<MODEL, 1, true, ATOM, TMA>(a, sh, B, n_poses, w, tpos, end, q1);
-    tpos += 32u;
-    if (more) q1[0] = n1[0];
+  pk_rows<MODEL, ATOM, TMA>(a, sh, B, n_poses, w, tpos, end);
+}
+
+// ---- tile ring: per warp, PK_RING shared-memory slots of one tile each, filled by cp.async -------------------------------
+// Every lane copies its own K rows of a tile (16-byte cp.async.cg: L2 -> shared memory, L1 left to the image gathers) and
+// later reads back exactly those rows, so a lane only waits for its own copies (cp.async.wait_group): no mbarrier, no
+// cross-lane handover, no uniform operands in the tile loop.  One commit group per tile (empty past the end of the pass);
+// the slot refilled at a step is the one read at the step before, whose rows the pose loop has consumed by then, so
+// PK_RING - 1 tiles are in flight while one is swept over the poses.
+
+// this lane's rows of one tile -> its rows of a slot, as one commit group (no copy when !valid: an empty group)
+template <int K>
+__device__ __forceinline__ void pk_ring_fill(unsigned int slot_lane, const float4* src_lane, bool valid) {
+  if (valid) {
+#pragma unroll
+    for (int j = 0; j < K; j++) asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(slot_lane + 512u * j), "l"(src_lane + 32 * j) : "memory");
   }
+  asm volatile("cp.async.commit_group;" ::: "memory");
+}
+
+// shared-memory address of this lane's first row in slot s of the calling warp's ring (recomputed from threadIdx where
+// needed: cheaper than keeping it in a register across the pose loop)
+template <int K>
+__device__ __forceinline__ unsigned int pk_ring_slot(const PkArgs& a, unsigned int smem_base, unsigned int s) {
+  return smem_base + a.ring_off + ((threadIdx.x >> 5) * PK_RING + s) * (32u * K * 16u) + 16u * (threadIdx.x & 31u);
+}
+
+__device__ __forceinline__ void sts_v4(unsigned int addr, uint4 v) {
+  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+__device__ __forceinline__ uint4 lds_v4(unsigned int addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
 }
 
 __device__ __forceinline__ float pk_tmax(const PkShared& sh, int n_poses) {
@@ -1013,6 +1074,11 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
   if (lane == 0) sh.q_cnt[warp] = 0;
   w.qn = 0;
   const unsigned int smem_base = static_cast<unsigned int>(__cvta_generic_to_shared(smem_hist));
+  // tile ring of this warp (interleaved split): this lane's rows of slot s at pk_ring_slot<K>(a, smem_base, s).  The pass's
+  // bookkeeping {next tile, tiles left, tile step, slot} lives in sh.ring_state[warp] (every lane writes the same values and
+  // reads them back).  While a tile is scored it waits there instead of in registers live across the pose loop.
+  constexpr bool RING = PK_TILE_RING && !TMA;
+  const unsigned int ring_state = static_cast<unsigned int>(__cvta_generic_to_shared(&sh.ring_state[warp]));
   const int n_items_per_batch = a.n_bags * (solve_mode ? PK_MAX_POSES : a.chunk);  // finalizer items of a full pose-list chunk
   const int fin_stride = max(1, static_cast<int>(gridDim.x) / (a.n_bags * PK_MAX_POSES));
 
@@ -1148,32 +1214,76 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
       // owning one region.  With contiguous slices the cost of a slice followed its region (deferred rechecks, histogram bin
       // collisions, cache hit rates), so the slowest block finished well after the median one, and every Nelder-Mead batch
       // waits for the slowest.  (Claiming tiles from an atomic counter was tried too: no better than the contiguous split
-      // at 256-point claims, and finer claims serialise on the counter.)  The next tile's rows are in flight while the current one is swept over the poses.
+      // at 256-point claims, and finer claims serialise on the counter.)
       constexpr unsigned int TP = 32u * K;
-      unsigned int tile = warp_global;
-      float4 qk[K];
-      bool full = static_cast<unsigned long long>(tile) * TP + TP <= bag_n;
-      if (full) pk_load_tile<K>(B.points, tile * TP, bag_n, lane, qk);
-      if (fresh) {
-        for (int i = t; i < a.copies * per_copy; i += PK_THREADS) smem_hist[i] = 0;
-        __syncthreads();
-      }
-      if (time_block) a.block_times[4 * blockIdx.x + 1] = global_ns();
-      while (full) {
-        const unsigned int ntile = tile + warps_total;
-        const bool nfull = static_cast<unsigned long long>(ntile) * TP + TP <= bag_n;
-        float4 nxt[K];
-        if (nfull) pk_load_tile<K>(B.points, ntile * TP, bag_n, lane, nxt);
-        pk_tile<MODEL, K, false, ATOM, TMA>(a, sh, B, n_poses, w, tile * TP, bag_n, qk);
-        tile = ntile;
-        full = nfull;
-        if (nfull) {
+      if constexpr (RING) {
+        // The warp's full tiles stream through its shared-memory ring, PK_RING - 1 of them in flight behind the one being
+        // scored.  Serpentine sweep: odd passes walk the warp's tiles backwards, so every pass begins on the tiles that the
+        // previous one touched last (still in L2 when the cloud is larger than L2) -- same tiles, other order, same counts.
+        {
+          const unsigned int n_full = bag_n / TP;
+          const unsigned int nt = warp_global < n_full ? (n_full - 1u - warp_global) / warps_total + 1u : 0u;
+          const bool backward = (batch & 1ull) != 0ull;
+          const unsigned int step = backward ? 0u - warps_total : warps_total;  // tiles between consecutive steps (mod 2^32)
+          const unsigned int tile0 = backward ? warp_global + (nt - 1u) * warps_total : warp_global;
 #pragma unroll
-          for (int j = 0; j < K; j++) qk[j] = nxt[j];
+          for (int s = 0; s + 1 < PK_RING; s++)
+            pk_ring_fill<K>(pk_ring_slot<K>(a, smem_base, s), B.points + static_cast<size_t>(tile0 + s * step) * TP + lane, static_cast<unsigned int>(s) < nt);
+          sts_v4(ring_state, make_uint4(tile0, nt, step, 0u));
         }
+        if (fresh) {
+          for (int i = t; i < a.copies * per_copy; i += PK_THREADS) smem_hist[i] = 0;
+          __syncthreads();
+        }
+        if (time_block) a.block_times[4 * blockIdx.x + 1] = global_ns();
+        for (;;) {
+          const uint4 rs = lds_v4(ring_state);  // {tile, tiles left, step, slot}
+          if (rs.y == 0u) break;
+          // this lane's copies of the tile landed (the later groups may still be in flight)
+          asm volatile("cp.async.wait_group %0;" ::"n"(PK_RING - 2) : "memory");
+          const unsigned int row0 = pk_ring_slot<K>(a, smem_base, rs.w);
+          float4 q[K];
+#pragma unroll
+          for (int j = 0; j < K; j++) {
+            asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(q[j].x), "=f"(q[j].y), "=f"(q[j].z), "=f"(q[j].w) : "r"(row0 + 512u * j) : "memory");
+          }
+          // refill the slot read at the step before (its rows went through the pose loop) with the tile PK_RING - 1 steps ahead
+          const unsigned int refill = rs.w == 0u ? PK_RING - 1u : rs.w - 1u;
+          pk_ring_fill<K>(pk_ring_slot<K>(a, smem_base, refill), B.points + static_cast<size_t>(rs.x + (PK_RING - 1) * rs.z) * TP + lane, rs.y > PK_RING - 1u);
+          sts_v4(ring_state, make_uint4(rs.x + rs.z, rs.y - 1u, rs.z, rs.w + 1u == PK_RING ? 0u : rs.w + 1u));
+          pk_tile<MODEL, K, false, ATOM, TMA>(a, sh, B, n_poses, w, rs.x * TP, bag_n, q);
+        }
+        // the cloud's ragged last tile (fewer than 32 * K points, register loads) belongs to the warp whose tile sequence reaches it
+        const unsigned int n_full = bag_n / TP;
+        if (n_full * TP < bag_n && n_full % warps_total == warp_global) pk_rows<MODEL, ATOM, TMA>(a, sh, B, n_poses, w, n_full * TP, bag_n);
+      } else {
+        // PK_TILE_RING=0 (A/B): the next tile's rows are in flight in registers while the current one is swept over the
+        // poses; every pass walks forwards
+        unsigned int tile = warp_global;
+        float4 qk[K];
+        bool full = static_cast<unsigned long long>(tile) * TP + TP <= bag_n;
+        if (full) pk_load_tile<K>(B.points, tile * TP, bag_n, lane, qk);
+        if (fresh) {
+          for (int i = t; i < a.copies * per_copy; i += PK_THREADS) smem_hist[i] = 0;
+          __syncthreads();
+        }
+        if (time_block) a.block_times[4 * blockIdx.x + 1] = global_ns();
+        while (full) {
+          const unsigned int ntile = tile + warps_total;
+          const bool nfull = static_cast<unsigned long long>(ntile) * TP + TP <= bag_n;
+          float4 nxt[K];
+          if (nfull) pk_load_tile<K>(B.points, ntile * TP, bag_n, lane, nxt);
+          pk_tile<MODEL, K, false, ATOM, TMA>(a, sh, B, n_poses, w, tile * TP, bag_n, qk);
+          tile = ntile;
+          full = nfull;
+          if (nfull) {
+#pragma unroll
+            for (int j = 0; j < K; j++) qk[j] = nxt[j];
+          }
+        }
+        // the cloud's ragged last tile (fewer than 32 * K points) belongs to whichever warp's sequence reaches it
+        if (static_cast<unsigned long long>(tile) * TP < bag_n) pk_range<MODEL, K, ATOM, TMA>(a, sh, B, n_poses, w, tile * TP, bag_n, qk, false);
       }
-      // the cloud's ragged last tile (fewer than 32 * K points) belongs to whichever warp's sequence reaches it
-      if (static_cast<unsigned long long>(tile) * TP < bag_n) pk_range<MODEL, K, ATOM, TMA>(a, sh, B, n_poses, w, tile * TP, bag_n, qk, false);
     }
     if (w.qn > 0) {
       pk_drain32<MODEL>(a, sh, B, w, 0, w.qn);
