@@ -131,6 +131,7 @@ def load_library():
     L.vlcal_nid_score_poses.argtypes = [C.POINTER(vp), C.c_int, dp, C.c_int, dp]
     L.vlcal_nid_set_poses_per_pass.argtypes = [vp, C.c_int]
     L.vlcal_nid_get_profile_passes.argtypes = [vp, C.POINTER(C.c_int64)]
+    L.vlcal_nid_get_profile_delta.argtypes = [vp, C.POINTER(C.c_int64)]
     L.vlcal_nid_debug_solve_stamps.argtypes = [vp, C.c_int, C.POINTER(C.c_uint64), ip]
     L.vlcal_nid_debug_block_times.argtypes = [vp, C.c_int, C.POINTER(C.c_uint64), ip]
     L.vlcal_nid_debug_tma_stats.argtypes = [vp, C.POINTER(C.c_uint64)]
@@ -151,6 +152,7 @@ def load_library():
     L.vlcal_nid_reorder_for_pose.argtypes = [vp, dp]
     L.vlcal_nid_filter_enabled.argtypes = [vp]
     L.vlcal_nid_debug_filter_check.argtypes = [vp, dp, C.c_int, C.POINTER(C.c_uint64), dp]
+    L.vlcal_nid_debug_filter_check_delta.argtypes = [vp, dp, C.c_int, C.POINTER(C.c_uint64), dp]
     L.vlcal_nid_p2p_create.argtypes = [C.c_int, C.c_int, C.c_int, C.POINTER(vp), vp]
     L.vlcal_nid_p2p_connect.argtypes = [vp, vp]
     L.vlcal_nid_p2p_attach.argtypes = [vp, vp]

@@ -115,12 +115,14 @@ class CostCalculatorNID:
     def filter_enabled(self) -> bool:
         return bool(self._L.vlcal_nid_filter_enabled(self._ctx))
 
-    def debug_filter_check(self, Ts):
-        """Test hook: (point_poses, deferred_to_exact, mismatches, max |uv32-uv64|/bound)."""
+    def debug_filter_check(self, Ts, delta=False):
+        """Test hook: (point_poses, deferred_to_exact, mismatches, max |uv32-uv64|/bound).  delta: equirectangular delta
+        step -- in every group of 8 poses, pose 0 is the anchor and the others are first-order updates from it."""
         Tc = T_to_colmajor(Ts)
         counts = (C.c_uint64 * 3)()
         ratio = C.c_double()
-        _lib.check(self._L.vlcal_nid_debug_filter_check(self._ctx, _dp(Tc), Tc.shape[0], counts, C.byref(ratio)))
+        fn = self._L.vlcal_nid_debug_filter_check_delta if delta else self._L.vlcal_nid_debug_filter_check
+        _lib.check(fn(self._ctx, _dp(Tc), Tc.shape[0], counts, C.byref(ratio)))
         return int(counts[0]), int(counts[1]), int(counts[2]), float(ratio.value)
 
     @property
@@ -137,10 +139,14 @@ class CostCalculatorNID:
         _lib.check(self._L.vlcal_nid_reset_profile(self._ctx))
 
     def profile(self):
-        launches, poses, ms, passes = C.c_int64(), C.c_int64(), C.c_double(), C.c_int64()
+        launches, poses, ms, passes, delta = C.c_int64(), C.c_int64(), C.c_double(), C.c_int64(), (C.c_int64 * 4)()
         _lib.check(self._L.vlcal_nid_get_profile(self._ctx, C.byref(launches), C.byref(ms), C.byref(poses)))
         _lib.check(self._L.vlcal_nid_get_profile_passes(self._ctx, C.byref(passes)))
-        return {"kernel_launches": launches.value, "kernel_ms_total": ms.value, "poses_total": poses.value, "passes": passes.value}
+        _lib.check(self._L.vlcal_nid_get_profile_delta(self._ctx, delta))
+        # persistent kernel: passes (and their poses) that took the equirectangular delta step; point-poses deferred to
+        # the exact path in the other passes and in the delta passes
+        return {"kernel_launches": launches.value, "kernel_ms_total": ms.value, "poses_total": poses.value, "passes": passes.value,
+                "delta_passes": delta[0], "delta_poses": delta[1], "deferred_plain": delta[2], "deferred_delta": delta[3]}
 
     def set_poses_per_pass(self, k: int):
         """Poses per pass over the cloud in pose-list evaluations (1..8, default 8); measurement hook, results unchanged."""

@@ -186,6 +186,18 @@ inline LeanCam make_lean_cam(const CameraParams& cam, const FastCam& f, int widt
     c.hx0 = dn(0.5 - cu);
     c.hy0 = dn(0.5 - cv);
     if (!(c.hx0 > 0.0f) || !(c.hy0 > 0.0f)) return c;
+    // delta step (lean_filter.cuh, above classify_lean_delta): terms 2-4 of its bound
+    const double su = W, sv = 2.0 * H;
+    c.eq_gu = static_cast<float>(su / (2.0 * M_PI));
+    c.eq_gv = static_cast<float>(sv / (2.0 * M_PI));
+    c.eq_ku = up(SAFETY * su / (4.0 * M_PI) * 1.15);
+    c.eq_kv = up(SAFETY * sv / (4.0 * M_PI) * 1.2072 * 1.15);
+    c.eq_lu = up(SAFETY * su / (2.0 * M_PI) / 8.07 * (1.0 + 1e-5));
+    c.eq_lv = up(SAFETY * sv / (2.0 * M_PI) / 8.07 * (1.0 + 1e-5));
+    c.eq_cu = up(SAFETY * (64.0 * U * su / (32.0 * M_PI) + 2.0 * U * (1.03 * W + 1.0)) + 1e-6);
+    c.eq_cv = up(SAFETY * (64.0 * U * sv / (32.0 * M_PI) + 2.0 * U * (1.03 * H + 1.0)) + 1e-6);
+    c.eq_hxd = dn(static_cast<double>(c.hx0) - static_cast<double>(c.eq_cu));
+    c.eq_nsx15 = dn(1.5 * static_cast<double>(c.nsfx));
   }
   c.enabled = 1;
   return c;

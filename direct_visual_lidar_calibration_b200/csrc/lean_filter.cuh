@@ -46,6 +46,13 @@ struct LeanCam {
   float hx0, hy0;         // 0.5 - cu, 0.5 - cv
   float nsfx, nsfy;       // -sfx, -sfy
   float eq_su, eq_sv;     // equirectangular: u' = lon_turns * W + cxh, v' = lat_turns * 2H + cyh
+  // equirectangular delta step (classify_lean_delta): gradient scales W / 2pi, 2H / 2pi; remainder, d-error and
+  // constant terms of its bound (derivation above classify_lean_delta)
+  float eq_gu, eq_gv;
+  float eq_ku, eq_kv;
+  float eq_lu, eq_lv;
+  float eq_cu, eq_cv;
+  float eq_hxd, eq_nsx15;  // hx0 - eq_cu and -1.5 sfx: the anchor's half-width hx is recomputed from delta and 1 / r_xz
 };
 
 // atan2(a, b) / (2 pi) in turns, (-0.5, 0.5]: octant reduction + odd minimax polynomial of degree 13 on [0, 1] (fitted for
@@ -115,6 +122,153 @@ VL_HD LeanVerdict lean_tail(const LeanCam& c, int width, float up, float vp, flo
   return v;
 }
 
+// ---- equirectangular: poses 1..P-1 of a batch as a first-order update from pose 0 (the anchor) -------------------------
+//
+// The poses of a Nelder-Mead batch lie close together (xr, xe, xc on a line through xo; the initial simplex x0 + 1e-3
+// along each axis), so for pose k the camera-frame point moves by D = p_k - p_0 = dR_k p + dt_k, dR_k = R_k - R_0,
+// dt_k = t_k - t_0, which is small against the point's distance from the camera's y axis r_xz.  The anchor step is the
+// plain classifier at pose 0 (same verdict) and keeps, per point, the projection (up0, vp0), its gradient g at the fp32
+// point q0 = p~_0, 1 / r_xz and a radius within which the guards of the plain classifier provably hold.  The delta step
+// projects pose k as  up = up0 + g_u . d,  vp = vp0 + g_v . d  with d = fl32(dR~_k p + dt~_k) (dR~, dt~ rounded once from
+// the double poses), a handful of FMAs instead of two rsqrt and two arctangents, and keeps the verdict only where
+// |up - u_ref(p_k) + 0.5| < 0.5 - |frac|, i.e. under the half-widths hx_k = hx_0 - (terms 2-4 below), as lean_tail tests.
+//
+// Soundness.  Let m = |D| + sqrt3 delta, so the ball B of radius m around q0 holds p_0 (|p_0 - q0| <= sqrt3 delta),
+// p_k and the segment between them.  With xi = p_0 - q0 and h a bound on the Hessian norm of u on B,
+//   u(p_k) - u(p_0) - grad u(q0) . D = int_0^1 (grad u(p_0 + sD) - grad u(q0)) . D ds,  |.| <= h (|xi||D| + |D|^2/2) <= h m^2/2.
+// The error of up splits into
+//   1. the anchor's own bound at pose 0 (0.5 - hx_0: the plain classifier's E, unchanged; hx_0 = hx0 - 1.5 sfx delta / r_xz
+//      is recomputed by the delta step in another rounding order, which the safety factor 2 of that term absorbs);
+//   2. the remainder h m^2 / 2.  lon = atan2(x, z) has Hessian norm 1 / r_xz^2.  lat = atan2(y, r_xz(x, z)): its Hessian
+//      is J^T H_2 J + phi_r grad^2 r_xz with J's rows (e_y, grad r_xz) orthonormal, |H_2| = 1 / n^2 (polar angle),
+//      |phi_r| = |y| / n^2 and |grad^2 r_xz| = 1 / r_xz, so |H_lat| <= (cos^2 b + |sin b| cos b) / r_xz^2 <= (1 + sqrt2) / 2
+//      / r_xz^2 (y = n sin b, r_xz = n cos b).  On B, r_xz >= r_xz(q0) - m >= (15/16 - 4e-7) r_xz~ because the delta
+//      step requires m < r_xz~ / 16, so 1 / r_xz,min^2 <= 1.138 / r_xz~^2; charged 1.15 (the fp32 1 / r_xz~^2 included).
+//      In pixels: eq_ku = S W / 4pi * 1.15, eq_kv = S 2H / 4pi * 1.2072 * 1.15 (S = 2, the safety factor of the anchor);
+//   3. the error of d: per component |d~ - D| <= 5u (sum_j |dR_ij| |p_j| + |dt_i|) (rounding of dR, dt and three FMAs);
+//      |p|_1 <= delta / 5.25u, so |d~ - D|_2 <= eps := 1.7 max|dR~| delta + 9u max|dt~|  (per pose: A, B of lean_delta_pose,
+//      both times 8.07).  It enters |D| <= |d~| + eps (hence m) and, through the gradient, |grad u| eps <= S W / 2pi eps / r_xz
+//      (|grad v| <= 2H / 2pi / |p| <= 2H / 2pi / r_xz): eq_lu, eq_lv.  This term is far below the others by construction
+//      (eps / r_xz ~ 1e-7 |dR|): no test can observe it, its charge rests on this derivation alone;
+//   4. the fp32 gradient (relative error <= 16u incl. MUFU.RSQ, charged 64u) times |d| <= r_xz / 16, the products of
+//      g . d, and the rounding of up0 + s at |up| <= 1.03 W + 1 (|s| <= W / 32pi): eq_cu = S (64u W / 32pi + 2u (1.03 W + 1))
+//      + 1e-6 (the reference's own double rounding, the rounding of hx_k), likewise eq_cv with 2H.
+// m^2 <= (1 + 1/64) |d~|^2 + 65 (eps + sqrt3 delta)^2 (the delta step computes it as fma(|d~|^2, 1.016, e8^2) with
+// e8 = 8.07 (eps + sqrt3 delta)).  Guards at pose k, all from  m < radius  (radius^2 kept per point, shrunk by 1e-4):
+//   * r_xz~ / 16: the remainder bound above; |p_k| >= 15/16 |q0| keeps n^2 > 2e-3 * 0.87 > 1e-3 (the reference's branch);
+//   * the seam: B must not meet the cut {x = 0, z <= 0} of atan2(x, z): distance r_xz~ if z~ > 0, else |x~|;
+//   * FoV: g = z - cos_fov |p| is 2-Lipschitz and the anchor's margin mf covers its fp32 and the reference's rounding,
+//     so g~_0 - mf > 2|D| keeps the pass at pose k (radius 0.49 (g~_0 - mf)) and -g~_0 - mf > 2|D| keeps the reject.
+// The anchor's own guards (n^2, r_xz > 40 delta, pole) must have held at pose 0 for a pass; otherwise the radius is 0
+// and the delta step defers every pose.  A NaN anywhere makes both predicates false: uncertain.
+struct LeanAnchor {
+  float up0, vp0;       // the anchor's projection (pixel coordinates minus 0.5)
+  float gux, guz;       // d up / d (x, z) of the camera-frame point, pixels per metre (lon has no y term)
+  float gvx, gvy, gvz;  // d vp / d (x, y, z)
+  float irxz;           // 1 / r_xz at the anchor
+  float hy;             // the anchor's half-width hy minus eq_cv (hx: hx0 - 1.5 sfx delta / r_xz, recomputed)
+  float rad2;           // > 0: pass radius^2; < 0: -(reject radius^2); 0: every pose k is uncertain
+};
+
+constexpr float LEAN_DELTA_SQ3 = 13.98f;   // 8.07 sqrt3
+constexpr float LEAN_DELTA_M2 = 1.016f;    // (1 + 1/64) and the rounding of |d~|^2
+
+// P: pose32 row of pose 0, as classify_lean.  Same operations as the plain classifier for the verdict.
+template <int MODEL>
+VL_HD LeanVerdict classify_lean_anchor(const FastCam& f, const LeanCam& c, int width, const float* __restrict__ P, float x, float y, float z, float delta, LeanAnchor& an) {
+  static_assert(MODEL == CAM_EQUIRECTANGULAR, "the delta step is derived for the equirectangular model");
+  const float pcx = fmaf(P[0], x, fmaf(P[1], y, fmaf(P[2], z, P[9])));
+  const float pcy = fmaf(P[3], x, fmaf(P[4], y, fmaf(P[5], z, P[10])));
+  const float pcz = fmaf(P[6], x, fmaf(P[7], y, fmaf(P[8], z, P[11])));
+  // u = W (0.5 + atan2(x, z) / 2pi),  v = H (0.5 + asin(y / |p|) / pi) = H (0.5 + 2 atan2(y, |(x, z)|) / 2pi)
+  // (equirectangular.hpp:21-27).  Input-error terms as validated in round 1 (project_fast): |d lon| <= 1.5 delta / rxz,
+  // |d asin| <= 1.03 (2.9 delta / |p| + 4u) |p| / rxz (an upper bound for the atan2 form as well, rxz <= |p|).
+  const float xx = pcx * pcx;
+  const float rxz2 = fmaf(pcz, pcz, xx);
+  const float n2 = fmaf(pcy, pcy, rxz2);
+  const float inv_n = LEAN_RSQRT(n2);
+  const float nrm = n2 * inv_n;
+  const float inv_rxz = LEAN_RSQRT(rxz2);
+  const float rxz = rxz2 * inv_rxz;
+  const float g = fmaf(-f.cos_fov, nrm, pcz);  // :32 (cos_fov = -1 for the full sphere: only the antipode is uncertain)
+  const float mf = fmaf(3.0f, delta, (12.0f * F32_U) * nrm);
+  const float lon = lean_atan2_turns(pcx, pcz);
+  const float lat = lean_atan2_turns(pcy, rxz);
+  const float up = fmaf(lon, c.eq_su, c.cxh);
+  const float vp = fmaf(lat, c.eq_sv, c.cyh);
+  const float t_lon = (1.5f * delta) * inv_rxz;
+  const float t_by = fmaf(2.9f * delta, inv_n, 4.0f * F32_U);
+  const float t_asn = (1.03f * t_by) * (nrm * inv_rxz);
+  const float hx = fmaf(c.nsfx, t_lon, c.hx0);
+  const float hy = fmaf(c.nsfy, t_asn, c.hy0);
+  // away from the |p|^2 < 1e-3 branch (:15), from the poles and from the seam's ill-conditioning
+  const bool ok = (n2 > 2e-3f) & (rxz > 40.0f * delta) & (rxz > 0.05f * nrm);
+  const bool pass = ok & (g > mf);
+  const bool rej = g < -mf;
+  // what the delta step needs: gradient (lon: (z, -x) / r_xz^2; lat: (-x y / r_xz, r_xz, -z y / r_xz) / n^2, per 2pi)
+  const float gu = c.eq_gu * (inv_rxz * inv_rxz);
+  const float gv = c.eq_gv * (inv_n * inv_n);
+  const float gvr = -(gv * pcy) * inv_rxz;
+  an.up0 = up, an.vp0 = vp;
+  an.gux = gu * pcz, an.guz = -(gu * pcx);
+  an.gvx = gvr * pcx, an.gvy = gv * rxz, an.gvz = gvr * pcz;
+  an.irxz = inv_rxz;
+  an.hy = hy - c.eq_cv;
+  const float r_seam = pcz > 0.0f ? rxz : fabsf(pcx);
+  const float r_pass = fminf(fminf(0.0625f * rxz, r_seam), 0.49f * (g - mf));
+  const float r_rej = 0.49f * (-g - mf);
+  an.rad2 = pass ? (0.9999f * r_pass) * r_pass : (rej ? -((0.9999f * r_rej) * r_rej) : 0.0f);
+  return lean_tail(c, width, up, vp, hx, hy, pass, rej);
+}
+
+// Q: pose k of the batch as written by lean_delta_pose: [dR row-major 9 | dt 3 | A | B], A, B: 8.07 eps = A delta + B
+template <int MODEL>
+VL_HD LeanVerdict classify_lean_delta(const LeanCam& c, int width, const float* __restrict__ Q, float x, float y, float z, float delta, const LeanAnchor& an) {
+  static_assert(MODEL == CAM_EQUIRECTANGULAR, "the delta step is derived for the equirectangular model");
+  const float dx = fmaf(Q[0], x, fmaf(Q[1], y, fmaf(Q[2], z, Q[9])));
+  const float dy = fmaf(Q[3], x, fmaf(Q[4], y, fmaf(Q[5], z, Q[10])));
+  const float dz = fmaf(Q[6], x, fmaf(Q[7], y, fmaf(Q[8], z, Q[11])));
+  const float nd2 = fmaf(dx, dx, fmaf(dy, dy, dz * dz));
+  const float e1 = fmaf(delta, Q[12], Q[13]);       // 8.07 eps
+  const float e8 = fmaf(delta, LEAN_DELTA_SQ3, e1);  // 8.07 (eps + sqrt3 delta)
+  const float m2 = fmaf(nd2, LEAN_DELTA_M2, e8 * e8);
+  const float up = an.up0 + fmaf(an.gux, dx, an.guz * dz);
+  const float vp = an.vp0 + fmaf(an.gvx, dx, fmaf(an.gvy, dy, an.gvz * dz));
+  const float r2m2 = (an.irxz * an.irxz) * m2;
+  const float lin = an.irxz * e1;
+  const float tlx = fmaf(-c.eq_lu, e1, c.eq_nsx15 * delta);  // -(input-error term of the anchor + term 3) * r_xz
+  const float hx = fmaf(-c.eq_ku, r2m2, fmaf(an.irxz, tlx, c.eq_hxd));
+  const float hy = fmaf(-c.eq_kv, r2m2, fmaf(-c.eq_lv, lin, an.hy));
+  const bool pass = m2 < an.rad2;
+  const bool rej = m2 < -an.rad2;
+  return lean_tail(c, width, up, vp, hx, hy, pass, rej);
+}
+
+// Spread of a batch for the delta step (a performance policy, not part of the bound): beyond it the remainder term would
+// defer too many point-poses, and the batch takes the plain classifier.  Nelder-Mead batches start at ~1e-3 and shrink.
+constexpr double LEAN_DELTA_MAX_DR = 4e-3;  // max |R_k - R_0| entry
+constexpr double LEAN_DELTA_MAX_DT = 2e-2;  // max |t_k - t_0| entry, metres
+
+// pose k of a batch relative to pose 0 (row-major 3x4 doubles) -> Q[16] for classify_lean_delta; true if within the spread
+VL_HD bool lean_delta_pose(const double* __restrict__ T, const double* __restrict__ T0, float* __restrict__ Q) {
+  float rmax = 0.0f, tmax = 0.0f;
+  for (int r = 0; r < 3; r++) {
+    for (int c = 0; c < 3; c++) {
+      Q[3 * r + c] = static_cast<float>(T[4 * r + c] - T0[4 * r + c]);
+      rmax = fmaxf(rmax, fabsf(Q[3 * r + c]));
+    }
+    Q[9 + r] = static_cast<float>(T[4 * r + 3] - T0[4 * r + 3]);
+    tmax = fmaxf(tmax, fabsf(Q[9 + r]));
+  }
+  // 8.07 (1.7 max|dR| delta + 9u max|dt|), rounded up by the 1e-3 margins
+  Q[12] = static_cast<float>(8.08 * 1.7 * static_cast<double>(rmax));
+  Q[13] = static_cast<float>(8.08 * 9.0 * static_cast<double>(F32_U) * static_cast<double>(tmax));
+  Q[14] = Q[15] = 0.0f;
+  bool close = true;
+  for (int i = 0; i < 12; i++) close = close && (fabsf(Q[i]) <= static_cast<float>(i < 9 ? LEAN_DELTA_MAX_DR : LEAN_DELTA_MAX_DT));
+  return close;
+}
+
 // P: pose32 row (R row-major 9, t 3); delta >= |pc_fp32 - pc_exact|_inf for this point and every pose of the batch
 template <int MODEL>
 VL_HD LeanVerdict classify_lean(const FastCam& f, const LeanCam& c, int width, const float* __restrict__ P, float x, float y, float z, float delta) {
@@ -152,32 +306,8 @@ VL_HD LeanVerdict classify_lean(const FastCam& f, const LeanCam& c, int width, c
     const bool rej = (base & (r2 > fmaf(c.K3, rho, c.T2hi))) | (pcz < -delta);
     return lean_tail(c, width, up, vp, hx, hy, pass, rej);
   } else if constexpr (MODEL == CAM_EQUIRECTANGULAR) {
-    // u = W (0.5 + atan2(x, z) / 2pi),  v = H (0.5 + asin(y / |p|) / pi) = H (0.5 + 2 atan2(y, |(x, z)|) / 2pi)
-    // (equirectangular.hpp:21-27).  Input-error terms as validated in round 1 (project_fast): |d lon| <= 1.5 delta / rxz,
-    // |d asin| <= 1.03 (2.9 delta / |p| + 4u) |p| / rxz (an upper bound for the atan2 form as well, rxz <= |p|).
-    const float xx = pcx * pcx;
-    const float rxz2 = fmaf(pcz, pcz, xx);
-    const float n2 = fmaf(pcy, pcy, rxz2);
-    const float inv_n = LEAN_RSQRT(n2);
-    const float nrm = n2 * inv_n;
-    const float inv_rxz = LEAN_RSQRT(rxz2);
-    const float rxz = rxz2 * inv_rxz;
-    const float g = fmaf(-f.cos_fov, nrm, pcz);  // :32 (cos_fov = -1 for the full sphere: only the antipode is uncertain)
-    const float mf = fmaf(3.0f, delta, (12.0f * F32_U) * nrm);
-    const float lon = lean_atan2_turns(pcx, pcz);
-    const float lat = lean_atan2_turns(pcy, rxz);
-    const float up = fmaf(lon, c.eq_su, c.cxh);
-    const float vp = fmaf(lat, c.eq_sv, c.cyh);
-    const float t_lon = (1.5f * delta) * inv_rxz;
-    const float t_by = fmaf(2.9f * delta, inv_n, 4.0f * F32_U);
-    const float t_asn = (1.03f * t_by) * (nrm * inv_rxz);
-    const float hx = fmaf(c.nsfx, t_lon, c.hx0);
-    const float hy = fmaf(c.nsfy, t_asn, c.hy0);
-    // away from the |p|^2 < 1e-3 branch (:15), from the poles and from the seam's ill-conditioning
-    const bool ok = (n2 > 2e-3f) & (rxz > 40.0f * delta) & (rxz > 0.05f * nrm);
-    const bool pass = ok & (g > mf);
-    const bool rej = g < -mf;
-    return lean_tail(c, width, up, vp, hx, hy, pass, rej);
+    LeanAnchor unused;
+    return classify_lean_anchor<MODEL>(f, c, width, P, x, y, z, delta, unused);
   } else {
     // other models: round-1 projection + bound (project_fast), FoV from |p| (these models need it anyway)
     const float n2 = fmaf(pcx, pcx, fmaf(pcy, pcy, pcz * pcz));

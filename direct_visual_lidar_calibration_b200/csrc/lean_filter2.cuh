@@ -115,6 +115,103 @@ struct LeanPacked {
   static constexpr bool value = MODEL == CAM_PLUMB_BOB || MODEL == CAM_EQUIRECTANGULAR;
 };
 
+// LeanAnchor of both points
+struct LeanAnchor2 {
+  F2 up0, vp0, gux, guz, gvx, gvy, gvz, irxz, hy, rad2;
+};
+
+// classify_lean_anchor for two points (also the equirectangular branch of classify_lean2)
+template <int MODEL>
+__device__ __forceinline__ LeanVerdict2 classify_lean2_anchor(const FastCam& f, const LeanCam& c, int width, const float* __restrict__ P, F2 X, F2 Y, F2 Z, F2 D, LeanAnchor2& an) {
+  static_assert(MODEL == CAM_EQUIRECTANGULAR, "the delta step is derived for the equirectangular model");
+  const F2 pcx = f2_fma(P[0], X, f2_fma(P[1], Y, f2_fma(P[2], Z, P[9])));
+  const F2 pcy = f2_fma(P[3], X, f2_fma(P[4], Y, f2_fma(P[5], Z, P[10])));
+  const F2 pcz = f2_fma(P[6], X, f2_fma(P[7], Y, f2_fma(P[8], Z, P[11])));
+  const F2 xx = f2_mul(pcx, pcx);
+  const F2 rxz2 = f2_fma(pcz, pcz, xx);
+  const F2 n2 = f2_fma(pcy, pcy, rxz2);
+  const F2 inv_n = f2_rsqrt(n2);
+  const F2 nrm = f2_mul(n2, inv_n);
+  const F2 inv_rxz = f2_rsqrt(rxz2);
+  const F2 rxz = f2_mul(rxz2, inv_rxz);
+  const F2 g = f2_fma(-f.cos_fov, nrm, pcz);
+  const F2 mf = f2_fma(3.0f, D, f2_mul(12.0f * F32_U, nrm));
+  const F2 lon = lean_atan2_turns2(pcx, pcz);
+  const F2 lat = lean_atan2_turns2(pcy, rxz);
+  const F2 up = f2_fma(lon, f2_dup(c.eq_su), c.cxh);
+  const F2 vp = f2_fma(lat, f2_dup(c.eq_sv), c.cyh);
+  const F2 t_lon = f2_mul(f2_mul(1.5f, D), inv_rxz);
+  const F2 t_by = f2_fma(f2_mul(2.9f, D), inv_n, 4.0f * F32_U);
+  const F2 t_asn = f2_mul(f2_mul(1.03f, t_by), f2_mul(nrm, inv_rxz));
+  const F2 hx = f2_fma(c.nsfx, t_lon, c.hx0);
+  const F2 hy = f2_fma(c.nsfy, t_asn, c.hy0);
+  const F2 far = f2_mul(40.0f, D), pole = f2_mul(0.05f, nrm);
+  // delta-step state (classify_lean_anchor)
+  const F2 gu = f2_mul(c.eq_gu, f2_mul(inv_rxz, inv_rxz));
+  const F2 gv = f2_mul(c.eq_gv, f2_mul(inv_n, inv_n));
+  const F2 gvr = f2_mul(f2_mul(-1.0f, f2_mul(gv, pcy)), inv_rxz);
+  an.up0 = up, an.vp0 = vp;
+  an.gux = f2_mul(gu, pcz), an.guz = f2_mul(-1.0f, f2_mul(gu, pcx));
+  an.gvx = f2_mul(gvr, pcx), an.gvy = f2_mul(gv, rxz), an.gvz = f2_mul(gvr, pcz);
+  an.irxz = inv_rxz;
+  an.hy = f2_add(hy, -c.eq_cv);
+  const F2 gm = f2_add(g, f2_mul(-1.0f, mf)), ngm = f2_fma(-1.0f, g, f2_mul(-1.0f, mf));  // g - mf, -g - mf
+  float n2s[2], rxzs[2], gs[2], mfs[2], fars[2], poles[2], pczs[2], pcxs[2], gms[2], ngms[2], rad2[2];
+  f2_unpack(n2, n2s[0], n2s[1]);
+  f2_unpack(rxz, rxzs[0], rxzs[1]);
+  f2_unpack(g, gs[0], gs[1]);
+  f2_unpack(mf, mfs[0], mfs[1]);
+  f2_unpack(far, fars[0], fars[1]);
+  f2_unpack(pole, poles[0], poles[1]);
+  f2_unpack(pcz, pczs[0], pczs[1]);
+  f2_unpack(pcx, pcxs[0], pcxs[1]);
+  f2_unpack(gm, gms[0], gms[1]);
+  f2_unpack(ngm, ngms[0], ngms[1]);
+  bool pass[2], rej[2];
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    const bool ok = (n2s[h] > 2e-3f) & (rxzs[h] > fars[h]) & (rxzs[h] > poles[h]);
+    pass[h] = ok & (gs[h] > mfs[h]);
+    rej[h] = gs[h] < -mfs[h];
+    const float r_seam = pczs[h] > 0.0f ? rxzs[h] : fabsf(pcxs[h]);
+    const float r_pass = fminf(fminf(0.0625f * rxzs[h], r_seam), 0.49f * gms[h]);
+    const float r_rej = 0.49f * ngms[h];
+    rad2[h] = pass[h] ? (0.9999f * r_pass) * r_pass : (rej[h] ? -((0.9999f * r_rej) * r_rej) : 0.0f);
+  }
+  an.rad2 = f2_pack(rad2[0], rad2[1]);
+  return lean_tail2(c, width, up, vp, hx, hy, pass, rej);
+}
+
+// classify_lean_delta for two points; Q: as written by lean_delta_pose
+template <int MODEL>
+__device__ __forceinline__ LeanVerdict2 classify_lean2_delta(const LeanCam& c, int width, const float* __restrict__ Q, F2 X, F2 Y, F2 Z, F2 D, const LeanAnchor2& an) {
+  static_assert(MODEL == CAM_EQUIRECTANGULAR, "the delta step is derived for the equirectangular model");
+  const F2 dx = f2_fma(Q[0], X, f2_fma(Q[1], Y, f2_fma(Q[2], Z, Q[9])));
+  const F2 dy = f2_fma(Q[3], X, f2_fma(Q[4], Y, f2_fma(Q[5], Z, Q[10])));
+  const F2 dz = f2_fma(Q[6], X, f2_fma(Q[7], Y, f2_fma(Q[8], Z, Q[11])));
+  const F2 nd2 = f2_fma(dx, dx, f2_fma(dy, dy, f2_mul(dz, dz)));
+  const F2 e1 = f2_fma(D, f2_dup(Q[12]), Q[13]);
+  const F2 e8 = f2_fma(D, f2_dup(LEAN_DELTA_SQ3), e1);
+  const F2 m2 = f2_fma(nd2, f2_dup(LEAN_DELTA_M2), f2_mul(e8, e8));
+  const F2 up = f2_add(an.up0, f2_fma(an.gux, dx, f2_mul(an.guz, dz)));
+  const F2 vp = f2_add(an.vp0, f2_fma(an.gvx, dx, f2_fma(an.gvy, dy, f2_mul(an.gvz, dz))));
+  const F2 r2m2 = f2_mul(f2_mul(an.irxz, an.irxz), m2);
+  const F2 lin = f2_mul(an.irxz, e1);
+  const F2 tlx = f2_fma(-c.eq_lu, e1, f2_mul(c.eq_nsx15, D));
+  const F2 hx = f2_fma(-c.eq_ku, r2m2, f2_fma(an.irxz, tlx, c.eq_hxd));
+  const F2 hy = f2_fma(-c.eq_kv, r2m2, f2_fma(-c.eq_lv, lin, an.hy));
+  float m2s[2], rads[2];
+  f2_unpack(m2, m2s[0], m2s[1]);
+  f2_unpack(an.rad2, rads[0], rads[1]);
+  bool pass[2], rej[2];
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    pass[h] = m2s[h] < rads[h];
+    rej[h] = m2s[h] < -rads[h];
+  }
+  return lean_tail2(c, width, up, vp, hx, hy, pass, rej);
+}
+
 // P: pose32 row as in classify_lean; X, Y, Z, D: coordinates and input-error bounds of the two points
 template <int MODEL>
 __device__ __forceinline__ LeanVerdict2 classify_lean2(const FastCam& f, const LeanCam& c, int width, const float* __restrict__ P, F2 X, F2 Y, F2 Z, F2 D) {
@@ -160,39 +257,8 @@ __device__ __forceinline__ LeanVerdict2 classify_lean2(const FastCam& f, const L
     }
     return lean_tail2(c, width, up, vp, hx, hy, pass, rej);
   } else {
-    const F2 xx = f2_mul(pcx, pcx);
-    const F2 rxz2 = f2_fma(pcz, pcz, xx);
-    const F2 n2 = f2_fma(pcy, pcy, rxz2);
-    const F2 inv_n = f2_rsqrt(n2);
-    const F2 nrm = f2_mul(n2, inv_n);
-    const F2 inv_rxz = f2_rsqrt(rxz2);
-    const F2 rxz = f2_mul(rxz2, inv_rxz);
-    const F2 g = f2_fma(-f.cos_fov, nrm, pcz);
-    const F2 mf = f2_fma(3.0f, D, f2_mul(12.0f * F32_U, nrm));
-    const F2 lon = lean_atan2_turns2(pcx, pcz);
-    const F2 lat = lean_atan2_turns2(pcy, rxz);
-    const F2 up = f2_fma(lon, f2_dup(c.eq_su), c.cxh);
-    const F2 vp = f2_fma(lat, f2_dup(c.eq_sv), c.cyh);
-    const F2 t_lon = f2_mul(f2_mul(1.5f, D), inv_rxz);
-    const F2 t_by = f2_fma(f2_mul(2.9f, D), inv_n, 4.0f * F32_U);
-    const F2 t_asn = f2_mul(f2_mul(1.03f, t_by), f2_mul(nrm, inv_rxz));
-    const F2 hx = f2_fma(c.nsfx, t_lon, c.hx0);
-    const F2 hy = f2_fma(c.nsfy, t_asn, c.hy0);
-    const F2 far = f2_mul(40.0f, D), pole = f2_mul(0.05f, nrm);
-    float n2s[2], rxzs[2], gs[2], mfs[2], fars[2], poles[2];
-    f2_unpack(n2, n2s[0], n2s[1]);
-    f2_unpack(rxz, rxzs[0], rxzs[1]);
-    f2_unpack(g, gs[0], gs[1]);
-    f2_unpack(mf, mfs[0], mfs[1]);
-    f2_unpack(far, fars[0], fars[1]);
-    f2_unpack(pole, poles[0], poles[1]);
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-      const bool ok = (n2s[h] > 2e-3f) & (rxzs[h] > fars[h]) & (rxzs[h] > poles[h]);
-      pass[h] = ok & (gs[h] > mfs[h]);
-      rej[h] = gs[h] < -mfs[h];
-    }
-    return lean_tail2(c, width, up, vp, hx, hy, pass, rej);
+    LeanAnchor2 unused;
+    return classify_lean2_anchor<MODEL>(f, c, width, P, X, Y, Z, D, unused);
   }
 }
 

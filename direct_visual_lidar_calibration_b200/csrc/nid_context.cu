@@ -956,6 +956,12 @@ int vlcal_nid_get_profile_passes(vlcal_nid_ctx* ctx, int64_t* passes) {
   return VLCAL_OK;
 }
 
+int vlcal_nid_get_profile_delta(vlcal_nid_ctx* ctx, int64_t stats[4]) {
+  if (!ctx || !stats) return VLCAL_ERR_INVALID_ARGUMENT;
+  for (int i = 0; i < 4; i++) stats[i] = ctx->delta_stats[i];
+  return VLCAL_OK;
+}
+
 int vlcal_nid_set_poses_per_pass(vlcal_nid_ctx* ctx, int poses_per_pass) {
   if (!ctx || poses_per_pass < 1 || poses_per_pass > PK_MAX_POSES) {
     set_last_error("poses_per_pass must be in [1, 8]");
@@ -1004,6 +1010,7 @@ int vlcal_nid_reset_profile(vlcal_nid_ctx* ctx) {
   ctx->launch_counter = 0;
   ctx->poses_total = 0;
   ctx->passes = 0;
+  for (int64_t& s : ctx->delta_stats) s = 0;
   ctx->kernel_ms_accum = 0.0;
   return VLCAL_OK;
 }
@@ -1159,13 +1166,17 @@ int vlcal_nid_filter_enabled(const vlcal_nid_ctx* ctx) {
   return ctx && ctx->fast.enabled && ctx->cloud->f32 ? 1 : 0;
 }
 
-int vlcal_nid_debug_filter_check(vlcal_nid_ctx* ctx, const double* T_camera_lidar, int n_poses, uint64_t counts[3], double* max_bound_ratio) {
+static int debug_filter_check(vlcal_nid_ctx* ctx, const double* T_camera_lidar, int n_poses, uint64_t counts[3], double* max_bound_ratio, bool delta) {
   if (!ctx || !T_camera_lidar || n_poses <= 0 || !counts) {
     set_last_error("invalid arguments");
     return VLCAL_ERR_INVALID_ARGUMENT;
   }
   if (!vlcal_nid_filter_enabled(ctx) || ctx->mode != VLCAL_NID_MODE_HISTOGRAM) {
     set_last_error("the fp32 filter is not enabled for this context (camera model / FoV / point layout)");
+    return VLCAL_ERR_UNSUPPORTED;
+  }
+  if (delta && (ctx->cam.model != CAM_EQUIRECTANGULAR || !ctx->lean.enabled || !PK_PACKED_FP32)) {
+    set_last_error("the delta step exists for the packed equirectangular classifier only");
     return VLCAL_ERR_UNSUPPORTED;
   }
   VL_CUDA(cudaSetDevice(ctx->device));
@@ -1199,7 +1210,9 @@ int vlcal_nid_debug_filter_check(vlcal_nid_ctx* ctx, const double* T_camera_lida
     a.dbg = d_dbg;
     const long long want_blocks = (a.n + NID_THREADS - 1) / NID_THREADS;
     const int grid = static_cast<int>(std::max<long long>(1, std::min<long long>(want_blocks, static_cast<long long>(ctx->num_sms) * 4)));
-    if (lean) {
+    if (delta) {
+      nid_lean_verify_kernel<CAM_EQUIRECTANGULAR, true><<<grid, NID_THREADS, 0, ctx->stream>>>(a, ctx->lean);
+    } else if (lean) {
       switch (ctx->cam.model) {
         case CAM_PLUMB_BOB: nid_lean_verify_kernel<CAM_PLUMB_BOB><<<grid, NID_THREADS, 0, ctx->stream>>>(a, ctx->lean); break;
         case CAM_FISHEYE: nid_lean_verify_kernel<CAM_FISHEYE><<<grid, NID_THREADS, 0, ctx->stream>>>(a, ctx->lean); break;
@@ -1225,6 +1238,14 @@ int vlcal_nid_debug_filter_check(vlcal_nid_ctx* ctx, const double* T_camera_lida
     *max_bound_ratio = f;
   }
   return VLCAL_OK;
+}
+
+int vlcal_nid_debug_filter_check(vlcal_nid_ctx* ctx, const double* T_camera_lidar, int n_poses, uint64_t counts[3], double* max_bound_ratio) {
+  return debug_filter_check(ctx, T_camera_lidar, n_poses, counts, max_bound_ratio, false);
+}
+
+int vlcal_nid_debug_filter_check_delta(vlcal_nid_ctx* ctx, const double* T_camera_lidar, int n_poses, uint64_t counts[3], double* max_bound_ratio) {
+  return debug_filter_check(ctx, T_camera_lidar, n_poses, counts, max_bound_ratio, true);
 }
 
 

@@ -122,6 +122,9 @@ struct vlcal_nid_ctx {
   int64_t launch_counter = 0;
   int64_t poses_total = 0;
   int64_t passes = 0;  // passes over the cloud (a persistent launch carries one per Nelder-Mead batch / pose chunk)
+  // persistent kernel: passes whose poses 1..P-1 took the equirectangular delta step, their poses, and the point-poses
+  // deferred to the exact path in the other passes / in those passes
+  int64_t delta_stats[4] = {0, 0, 0, 0};
   double kernel_ms_accum = 0.0;
   // debug: globaltimer stamps of the persistent kernel's batches (vlcal_nid_debug_solve_stamps)
   int pk_chunk = 8;  // poses per pass of the persistent kernel's pose-list mode (vlcal_nid_set_poses_per_pass)

@@ -89,11 +89,14 @@ static int pk_make_tensor_map(const uint8_t* img, int width, int height, PkTenso
   return VLCAL_OK;
 }
 
-static PkKernel pk_pick(int model, int k) {
+// delta: the launch may carry equirectangular batches of nearby poses (the instance with the delta step, K = 2)
+static PkKernel pk_pick(int model, int k, bool delta = false) {
   static const int atom = [] {
     const char* e = std::getenv("VLCAL_PK_ATOM");
     return e ? (std::atoi(e) != 0 ? 1 : 0) : 0;
   }();
+  if (PK_DELTA_POSES && delta && model == CAM_EQUIRECTANGULAR && pk_kernel_k(model, k) == 2)
+    return atom ? nid_persistent_kernel<CAM_EQUIRECTANGULAR, 2, 1, false, true> : nid_persistent_kernel<CAM_EQUIRECTANGULAR, 2, 0, false, true>;
   switch (model) {
     case CAM_PLUMB_BOB: return pk_pick_ka<CAM_PLUMB_BOB>(k, atom);
     case CAM_FISHEYE: return pk_pick_ka<CAM_FISHEYE>(k, atom);
@@ -195,7 +198,7 @@ struct PinBuf {
 
 // device scratch of one launch, one allocation, zeroed by one memset
 struct PkScratchLayout {
-  size_t ghist, gmarg, arrive, fin_done, tile_next, abort_flag, seq, tma_stats, box, solve, total;
+  size_t ghist, gmarg, arrive, fin_done, tile_next, abort_flag, seq, tma_stats, delta_stats, box, solve, total;
   PkScratchLayout(int n_bags, int nb) {
     size_t o = 0;
     auto take = [&](size_t bytes) {
@@ -211,6 +214,7 @@ struct PkScratchLayout {
     abort_flag = take(sizeof(unsigned int));
     seq = take(sizeof(unsigned long long));
     tma_stats = take(sizeof(unsigned long long) * 2);
+    delta_stats = take(sizeof(unsigned long long) * 4);
     box = take(sizeof(PkMailbox));
     solve = take(sizeof(PkSolve));
     total = o;
@@ -251,6 +255,7 @@ void pk_fill_common(PkArgs& a, vlcal_nid_ctx* const* ctxs, int n_ctxs, const PkG
   a.abort_flag = reinterpret_cast<unsigned int*>(scratch + L.abort_flag);
   a.seq_counter = reinterpret_cast<unsigned long long*>(scratch + L.seq);
   a.box[0] = reinterpret_cast<PkMailbox*>(scratch + L.box);
+  a.delta_stats = reinterpret_cast<unsigned long long*>(scratch + L.delta_stats);
   a.world = 1, a.rank = 0;
   a.timeout_ns = pk_timeout_ns();
 }
@@ -275,7 +280,7 @@ int pk_solve(
   long long total_points = 0;
   for (int i = 0; i < n_ctxs; i++) total_points += ctxs[i]->cloud->n;
   const int kpt = pk_points_per_lane(c0, total_points);
-  PkKernel kernel = pk_pick(c0->cam.model, kpt);
+  PkKernel kernel = pk_pick(c0->cam.model, kpt, true);  // Nelder-Mead batches close in as the simplex shrinks
   // TMA variant (A/B): image windows staged in shared memory; needs 16-byte row pitches and 128-byte aligned histogram copies
   const size_t hist_bytes = static_cast<size_t>(std::max<size_t>(1, std::min<size_t>(PK_WARPS / 4, (64 * 1024) / (static_cast<size_t>(PK_MAX_POSES) * c0->bins * c0->bins * 4)))) * PK_MAX_POSES * c0->bins * c0->bins * 4;
   const bool use_tma = pk_tma_requested() != 0 && pk_pick_tma(c0->cam.model, kpt) != nullptr && c0->image->width % 16 == 0 && hist_bytes % 128 == 0;
@@ -411,6 +416,8 @@ int pk_solve(
   // scratch goes back to the pool: the kernel has published its last word, nothing else is enqueued on it
   VL_CUDA(cudaStreamSynchronize(c0->stream));
   if (use_tma) VL_CUDA(cudaMemcpy(c0->pk_tma_stats, sp + L.tma_stats, sizeof(c0->pk_tma_stats), cudaMemcpyDeviceToHost));
+  unsigned long long delta_stats[4];
+  VL_CUDA(cudaMemcpy(delta_stats, sp + L.delta_stats, sizeof(delta_stats), cudaMemcpyDeviceToHost));
 
   const NmMachine& fin = h_result->nm;
   // the objective's side effects in the reference's evaluation order (:112-116)
@@ -445,6 +452,7 @@ int pk_solve(
   // profile: one launch carried `batches` passes over the cloud(s)
   c0->launches += 1;
   c0->passes += static_cast<int64_t>(h_result->batches);
+  for (int i = 0; i < 4; i++) c0->delta_stats[i] += static_cast<int64_t>(delta_stats[i]);
   c0->poses_total += static_cast<int64_t>(h_result->poses);
   return VLCAL_OK;
 }
@@ -457,7 +465,26 @@ int pk_score_poses(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_colma
   long long total_points = 0;
   for (int i = 0; i < n_ctxs; i++) total_points += ctxs[i]->cloud->n;
   const int kpt = pk_points_per_lane(c0, total_points);
-  PkKernel kernel = pk_pick(c0->cam.model, kpt);
+  // the instance with the delta step only when some chunk of the list lies within its gate (the kernel checks every
+  // chunk again); widely spread lists and one-pose chunks keep the plain instance
+  bool delta = false;
+  if (c0->cam.model == CAM_EQUIRECTANGULAR) {
+    const int ch = std::max(1, std::min(PK_MAX_POSES, c0->pk_chunk));
+    auto rows = [&](int p, double* R) {
+      for (int r = 0; r < 3; r++)
+        for (int c = 0; c < 4; c++) R[4 * r + c] = T_colmajor[16 * static_cast<size_t>(p) + r + 4 * c];
+    };
+    for (int b = 0; b < n_poses && !delta; b += ch) {
+      const int cnt = std::min(ch, n_poses - b);
+      double R0[12], Rk[12];
+      float Q[16];
+      rows(b, R0);
+      bool close = cnt >= 2;
+      for (int k = 1; k < cnt && close; k++) rows(b + k, Rk), close = lean_delta_pose(Rk, R0, Q);
+      delta = close;
+    }
+  }
+  PkKernel kernel = pk_pick(c0->cam.model, kpt, delta);
   PkGeom g;
   {
     const int rc = pk_geometry(c0->device, c0->num_sms, kernel, c0->bins * c0->bins, pk_kernel_k(c0->cam.model, kpt), &g);
@@ -518,6 +545,8 @@ int pk_score_poses(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_colma
   double* hscore = static_cast<double*>(host.p);
   VL_CUDA(cudaMemcpyAsync(hscore, d_scores.p, sizeof(double) * score_count, cudaMemcpyDeviceToHost, c0->stream));
   if (hist_out) VL_CUDA(cudaMemcpyAsync(hist_out, d_hist.p, sizeof(int) * static_cast<size_t>(n_poses) * nb, cudaMemcpyDeviceToHost, c0->stream));
+  unsigned long long delta_stats[4];
+  VL_CUDA(cudaMemcpyAsync(delta_stats, static_cast<char*>(scratch.p) + L.delta_stats, sizeof(delta_stats), cudaMemcpyDeviceToHost, c0->stream));
   VL_CUDA(cudaStreamSynchronize(c0->stream));
   if (*h_error) {
     set_last_error("persistent evaluation: a wait timed out (grid not co-resident?)");
@@ -534,6 +563,7 @@ int pk_score_poses(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_colma
   }
   c0->launches += 1;
   c0->passes += n_chunks;
+  for (int i = 0; i < 4; i++) c0->delta_stats[i] += static_cast<int64_t>(delta_stats[i]);
   c0->poses_total += n_poses;
   return VLCAL_OK;
 }

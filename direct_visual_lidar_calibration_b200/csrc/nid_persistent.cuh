@@ -81,6 +81,11 @@ struct alignas(64) PkTensorMap {         // a CUtensorMap (cuTensorMapEncodeTile
 #define PK_RING_SLOTS 2  // PK_RING_SLOTS - 1 tiles in flight; every slot more takes 24 KB of the SM's L1 for shared memory
 #endif
 constexpr int PK_RING = PK_RING_SLOTS;
+// Equirectangular batches of nearby poses: poses 1..P-1 as first-order updates from pose 0 (classify_lean2_delta);
+// 0: every pose through the plain classifier (A/B build)
+#ifndef PK_DELTA_POSES
+#define PK_DELTA_POSES 1
+#endif
 static_assert(PK_RING >= 2 && PK_RING <= 8, "PK_RING_SLOTS: 2..8 tile slots per warp");
 // dynamic shared memory of the block's tile rings: PK_WARPS x PK_RING slots of one 32*k-point tile (float4 rows)
 __host__ __device__ constexpr unsigned int pk_ring_bytes(int k) { return PK_TILE_RING ? static_cast<unsigned int>(PK_WARPS * PK_RING * 32 * k * 16) : 0u; }
@@ -150,6 +155,9 @@ struct PkArgs {
   unsigned long long* stamps;       // optional [cap][PK_STAMP_SLOTS] globaltimer stamps per batch
   int stamps_cap;
   unsigned long long* tma_stats;    // TMA variant: [0] gathers served from the shared-memory window, [1] gathers that escaped it
+  // [4]: passes (batches / chunks) that took the delta step and their poses (block 0), point-poses deferred to the exact
+  // path in the other passes and in those passes (every block)
+  unsigned long long* delta_stats;
   unsigned long long* block_times;  // optional [grid][4]: every block's {enter, hist zeroed, main loop done, arrived} stamps of batch block_times_batch
   int block_times_batch;
 };
@@ -159,6 +167,8 @@ struct PkShared {
   double init_T[16];
   double pose64[PK_MAX_POSES][12];
   float4 pose32[PK_MAX_POSES][4];  // rows: [R00 R01 R02 t0] [R10 R11 R12 t1] [R20 R21 R22 t2] [max|t| 0 0 0]
+  float4 dpose[PK_MAX_POSES][4];   // poses 1..P-1 relative to pose 0, as lean_delta_pose writes them (delta step)
+  int delta_on;                    // the batch takes the delta step (block-uniform)
   double ys[PK_MAX_POSES];
   double parts[PK_MAX_WORDS];
   double fin_out[PK_WARPS];  // NIDs of the items one finalizer round covers (Nelder-Mead mode)
@@ -178,6 +188,7 @@ struct PkShared {
   unsigned char q_pose[PK_WARPS][PK_QUEUE];
   int q_cnt[PK_WARPS];  // fill count of each warp's queue
   uint4 ring_state[PK_WARPS];  // tile ring bookkeeping of each warp: {next tile, tiles left in the pass, tile step, slot}
+  unsigned int deferred[PK_WARPS][2];  // point-poses each warp deferred to the exact path: plain passes, delta passes
 };
 
 // ---- small PTX helpers ---------------------------------------------------------------------------------------------
@@ -548,6 +559,17 @@ __device__ __forceinline__ void pk_pose_from_list(PkShared& sh, int k, const dou
   sh.pose32[k][3] = make_float4(nextafterf(static_cast<float>(tmax), INFINITY), 0.f, 0.f, 0.f);
 }
 
+// warp 0, once the batch's n poses are in sh.pose64: the rows of the delta step and the batch's gate (every pose within
+// lean_delta_pose's spread of pose 0, and at least two poses)
+__device__ __forceinline__ void pk_delta_rows(PkShared& sh, int n, int lane) {
+  __syncwarp();
+  bool close = true;
+  if (lane >= 1 && lane < n) close = lean_delta_pose(sh.pose64[lane], sh.pose64[0], &sh.dpose[lane][0].x);
+  const bool on = __all_sync(0xffffffffu, close) && n >= 2;
+  if (lane == 0) sh.delta_on = on ? 1 : 0;
+  __syncwarp();
+}
+
 // ---- block-uniform waits with a timeout ------------------------------------------------------------------------------
 
 // thread 0 spins until *counter >= expected; returns false (for every thread) if the launch is being aborted
@@ -804,7 +826,8 @@ __device__ __forceinline__ void pk_drain32(const PkArgs& a, const PkShared& sh, 
 // one tile = 32*K consecutive points starting at `tile`, swept over the P poses of the batch; the image-bin gathers of
 // pose p stay in flight while pose p+1 is classified and are consumed by the histogram increments one iteration later.
 // PARTIAL: the tile may reach past `end` (only the single-row tiles at the end of a warp's slice).
-template <int MODEL, int K, bool PARTIAL, int ATOM, bool TMA>
+// DPOSE: the kernel instance carries the equirectangular delta step (nid_persistent_kernel).
+template <int MODEL, int K, bool PARTIAL, int ATOM, bool TMA, bool DPOSE = false>
 __device__ __forceinline__ void pk_tile(const PkArgs& a, const PkShared& sh, const PkBagRegs& B, int n_poses, PkWarp& w, unsigned int tile, unsigned int end, const float4 (&q)[K]) {
   float px[K], py[K], pz[K], dl[K];
   unsigned int lb[K];
@@ -831,64 +854,105 @@ __device__ __forceinline__ void pk_tile(const PkArgs& a, const PkShared& sh, con
 #pragma unroll
   for (int j = 0; j < K; j++) pend_bin[j] = -1, pend_inc[j] = 0;
   unsigned int pend_off = 0;
-  for (int p = 0; p <= n_poses; p++) {
-    bool acc[K];
-    int pix[K], wx[K], wy[K];
-    if (p < n_poses) {
-      const float4 r0 = sh.pose32[p][0], r1 = sh.pose32[p][1], r2 = sh.pose32[p][2];
-      const float Pm[12] = {r0.x, r0.y, r0.z, r1.x, r1.y, r1.z, r2.x, r2.y, r2.z, r0.w, r1.w, r2.w};
-      if constexpr (PACKED) {
+  // :49 hist(image_bin, lidar_bin)++ for the previous pose's verdicts
+  auto count_previous = [&]() {
 #pragma unroll
-        for (int j = 0; j < K; j += 2) {  // two points per instruction on the packed fp32 pipe (lean_filter2.cuh)
-          const LeanVerdict2 v = classify_lean2<MODEL>(a.fast, a.lean, a.width, Pm, X2[j / 2], Y2[j / 2], Z2[j / 2], D2[j / 2]);
-#pragma unroll
-          for (int h = 0; h < 2; h++) {
-            acc[j + h] = v.accept[h];
-            if (v.uncertain[h]) unc_mask |= unc_bit << (j + h);
-            pix[j + h] = v.idx[h];
-            if constexpr (TMA) wx[j + h] = v.ixb[h], wy[j + h] = v.iyb[h];
-          }
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < K; j++) {
-          const LeanVerdict v = classify_lean<MODEL>(a.fast, a.lean, a.width, Pm, px[j], py[j], pz[j], dl[j]);
-          acc[j] = PARTIAL ? (v.accept & valid0) : v.accept;
-          const bool unc = PARTIAL ? (v.uncertain & valid0) : v.uncertain;
-          if (unc) unc_mask |= unc_bit << j;
-          pix[j] = v.idx;
-          if constexpr (TMA) wx[j] = v.ixb, wy[j] = v.iyb;
-        }
-      }
-      unc_bit <<= K;
-    }
-#pragma unroll
-    for (int j = 0; j < K; j++) {  // :49 hist(image_bin, lidar_bin)++ for the previous pose
+    for (int j = 0; j < K; j++) {
       if constexpr (ATOM == 0) {
         if (pend_bin[j] >= 0) red_shared_inc(lb[j] + pend_off + 4u * static_cast<unsigned int>(pend_bin[j]));
       } else {
         red_shared_add(lb[j] + pend_off + 4u * static_cast<unsigned int>(pend_bin[j]), pend_inc[j]);
       }
     }
-    if (p < n_poses) {
-      pend_off = 4u * static_cast<unsigned int>(p * a.nb);
+  };
+  // the image-bin gathers of pose p's accepted verdicts, consumed by count_previous one pose later
+  auto gather = [&](int p, const bool (&acc)[K], const int (&pix)[K], const int (&wx)[K], const int (&wy)[K]) {
+    pend_off = 4u * static_cast<unsigned int>(p * a.nb);
 #pragma unroll
-      for (int j = 0; j < K; j++) {
-        if constexpr (TMA) {
-          const unsigned int dx = static_cast<unsigned int>(wx[j] - w.win_x0b), dy = static_cast<unsigned int>(wy[j] - w.win_y0b);
-          const bool inw = acc[j] & (dx < w.win_w) & (dy < w.win_h);
-          const bool out = acc[j] & !inw;
-          pend_bin[j] = gather_u8_window(inw, out, w.win_addr + dy * w.win_w + dx, B.bin_image + pix[j], ATOM == 0 ? -1 : 0);
-          if constexpr (ATOM != 0) pend_inc[j] = acc[j] ? 1 : 0;
-          w.n_window += inw ? 1u : 0u;
-          w.n_escaped += out ? 1u : 0u;
-        } else if constexpr (ATOM == 0) {
-          pend_bin[j] = ldg_u8_or_neg(acc[j], B.bin_image + pix[j]);
-        } else {
-          pend_bin[j] = ldg_u8_or_zero(acc[j], B.bin_image + pix[j]);
-          pend_inc[j] = acc[j] ? 1 : 0;
-        }
+    for (int j = 0; j < K; j++) {
+      if constexpr (TMA) {
+        const unsigned int dx = static_cast<unsigned int>(wx[j] - w.win_x0b), dy = static_cast<unsigned int>(wy[j] - w.win_y0b);
+        const bool inw = acc[j] & (dx < w.win_w) & (dy < w.win_h);
+        const bool out = acc[j] & !inw;
+        pend_bin[j] = gather_u8_window(inw, out, w.win_addr + dy * w.win_w + dx, B.bin_image + pix[j], ATOM == 0 ? -1 : 0);
+        if constexpr (ATOM != 0) pend_inc[j] = acc[j] ? 1 : 0;
+        w.n_window += inw ? 1u : 0u;
+        w.n_escaped += out ? 1u : 0u;
+      } else if constexpr (ATOM == 0) {
+        pend_bin[j] = ldg_u8_or_neg(acc[j], B.bin_image + pix[j]);
+      } else {
+        pend_bin[j] = ldg_u8_or_zero(acc[j], B.bin_image + pix[j]);
+        pend_inc[j] = acc[j] ? 1 : 0;
       }
+    }
+  };
+  // verdicts of points j, j + 1 from the packed classifier
+  auto record2 = [&](const LeanVerdict2& v, int j, bool (&acc)[K], int (&pix)[K], int (&wx)[K], int (&wy)[K]) {
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      acc[j + h] = v.accept[h];
+      if (v.uncertain[h]) unc_mask |= unc_bit << (j + h);
+      pix[j + h] = v.idx[h];
+      if constexpr (TMA) wx[j + h] = v.ixb[h], wy[j + h] = v.iyb[h];
+    }
+  };
+  // Equirectangular batches whose poses lie close together (sh.delta_on, set with the poses): pose 0 is the anchor, poses
+  // 1..P-1 are first-order updates from it (classify_lean2_delta; bound and guards in lean_filter.cuh)
+  constexpr bool DELTA = DPOSE && PK_DELTA_POSES && PACKED && MODEL == CAM_EQUIRECTANGULAR && !TMA;
+  const bool delta_tile = DELTA && sh.delta_on;
+  if (delta_tile) {
+    if constexpr (DELTA) {
+      LeanAnchor2 an[K / 2];
+      {
+        bool acc[K];
+        int pix[K], wx[K], wy[K];
+        const float4 r0 = sh.pose32[0][0], r1 = sh.pose32[0][1], r2 = sh.pose32[0][2];
+        const float Pm[12] = {r0.x, r0.y, r0.z, r1.x, r1.y, r1.z, r2.x, r2.y, r2.z, r0.w, r1.w, r2.w};
+#pragma unroll
+        for (int j = 0; j < K; j += 2)
+          record2(classify_lean2_anchor<MODEL>(a.fast, a.lean, a.width, Pm, X2[j / 2], Y2[j / 2], Z2[j / 2], D2[j / 2], an[j / 2]), j, acc, pix, wx, wy);
+        unc_bit <<= K;
+        gather(0, acc, pix, wx, wy);
+      }
+      for (int p = 1; p < n_poses; p++) {
+        bool acc[K];
+        int pix[K], wx[K], wy[K];
+        const float4 q0 = sh.dpose[p][0], q1 = sh.dpose[p][1], q2 = sh.dpose[p][2], q3 = sh.dpose[p][3];
+        const float Q[14] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, q3.x, q3.y};
+#pragma unroll
+        for (int j = 0; j < K; j += 2) record2(classify_lean2_delta<MODEL>(a.lean, a.width, Q, X2[j / 2], Y2[j / 2], Z2[j / 2], D2[j / 2], an[j / 2]), j, acc, pix, wx, wy);
+        unc_bit <<= K;
+        count_previous();
+        gather(p, acc, pix, wx, wy);
+      }
+      count_previous();
+    }
+  } else {
+    for (int p = 0; p <= n_poses; p++) {
+      bool acc[K];
+      int pix[K], wx[K], wy[K];
+      if (p < n_poses) {
+        const float4 r0 = sh.pose32[p][0], r1 = sh.pose32[p][1], r2 = sh.pose32[p][2];
+        const float Pm[12] = {r0.x, r0.y, r0.z, r1.x, r1.y, r1.z, r2.x, r2.y, r2.z, r0.w, r1.w, r2.w};
+        if constexpr (PACKED) {
+#pragma unroll
+          for (int j = 0; j < K; j += 2)  // two points per instruction on the packed fp32 pipe (lean_filter2.cuh)
+            record2(classify_lean2<MODEL>(a.fast, a.lean, a.width, Pm, X2[j / 2], Y2[j / 2], Z2[j / 2], D2[j / 2]), j, acc, pix, wx, wy);
+        } else {
+#pragma unroll
+          for (int j = 0; j < K; j++) {
+            const LeanVerdict v = classify_lean<MODEL>(a.fast, a.lean, a.width, Pm, px[j], py[j], pz[j], dl[j]);
+            acc[j] = PARTIAL ? (v.accept & valid0) : v.accept;
+            const bool unc = PARTIAL ? (v.uncertain & valid0) : v.uncertain;
+            if (unc) unc_mask |= unc_bit << j;
+            pix[j] = v.idx;
+            if constexpr (TMA) wx[j] = v.ixb, wy[j] = v.iyb;
+          }
+        }
+        unc_bit <<= K;
+      }
+      count_previous();
+      if (p < n_poses) gather(p, acc, pix, wx, wy);
     }
   }
   // Deferred (point, pose) pairs of this tile -> the warp's queue for the exact path.  Doing this once per tile instead of inside the pose loop
@@ -898,6 +962,7 @@ __device__ __forceinline__ void pk_tile(const PkArgs& a, const PkShared& sh, con
   // Otherwise: one ballot per round.
   const int cnt = __popc(unc_mask);
   const int total = __reduce_add_sync(0xffffffffu, cnt);
+  if (w.lane == 0 && total > 0) atoms_add(static_cast<unsigned int>(__cvta_generic_to_shared(&sh.deferred[threadIdx.x >> 5][delta_tile ? 1 : 0])), total);
   if (total > 0 && total <= 32) {
     if (w.qn + total > PK_QUEUE) {  // make room first (qn > 32 here): the last 32 queued pairs go to the exact path now
       pk_drain32<MODEL>(a, sh, B, w, w.qn - 32, 32);
@@ -1040,7 +1105,10 @@ __device__ __forceinline__ void pk_stamp(const PkArgs& a, unsigned long long bat
 // stamps per batch: 0 block 0 enters the batch, 1 block 0 main loop done, 2 block 0 merged + arrived,
 //                   3 finalizer of item 0: all blocks arrived, 4 finalizer of item 0: score published,
 //                   5 block 0: all scores seen, 7 block 0: Nelder-Mead machine stepped, 6 block 0: next poses ready
-template <int MODEL, int K, int ATOM, bool TMA = false>
+// DPOSE: this instance carries the equirectangular delta step (instantiated for equirectangular, K = 2 only; the host
+// picks it for Nelder-Mead solves and for pose lists with a chunk inside the gate, see pk_pick).  Its anchor state costs
+// registers in the whole kernel, so the plain instance stays for everything else.
+template <int MODEL, int K, int ATOM, bool TMA = false, bool DPOSE = false>
 __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kernel(const __grid_constant__ PkArgs a) {
   extern __shared__ __align__(128) int smem_hist[];
   __shared__ PkShared sh;
@@ -1071,13 +1139,14 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
   w.q_idx = static_cast<unsigned int>(__cvta_generic_to_shared(sh.q_idx[warp]));
   w.q_pose = static_cast<unsigned int>(__cvta_generic_to_shared(sh.q_pose[warp]));
   w.q_cnt = static_cast<unsigned int>(__cvta_generic_to_shared(&sh.q_cnt[warp]));
-  if (lane == 0) sh.q_cnt[warp] = 0;
+  if (lane == 0) sh.q_cnt[warp] = 0, sh.deferred[warp][0] = sh.deferred[warp][1] = 0u;
   w.qn = 0;
   const unsigned int smem_base = static_cast<unsigned int>(__cvta_generic_to_shared(smem_hist));
   // tile ring of this warp (interleaved split): this lane's rows of slot s at pk_ring_slot<K>(a, smem_base, s).  The pass's
   // bookkeeping {next tile, tiles left, tile step, slot} lives in sh.ring_state[warp] (every lane writes the same values and
   // reads them back).  While a tile is scored it waits there instead of in registers live across the pose loop.
   constexpr bool RING = PK_TILE_RING && !TMA;
+  constexpr bool DELTA = DPOSE && PK_DELTA_POSES && PK_PACKED_FP32 && MODEL == CAM_EQUIRECTANGULAR && K % 2 == 0 && !TMA && PK_TILE_RING;  // as in pk_tile
   const unsigned int ring_state = static_cast<unsigned int>(__cvta_generic_to_shared(&sh.ring_state[warp]));
   const int n_items_per_batch = a.n_bags * (solve_mode ? PK_MAX_POSES : a.chunk);  // finalizer items of a full pose-list chunk
   const int fin_stride = max(1, static_cast<int>(gridDim.x) / (a.n_bags * PK_MAX_POSES));
@@ -1090,11 +1159,15 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
     for (int i = t; i < static_cast<int>(sizeof(NmMachine) / 8); i += PK_THREADS) dst[i] = src[i];
     if (t < 16) sh.init_T[t] = a.solve->init_T[t];
     __syncthreads();
-    if (warp == 0) pk_poses_of_candidates(sh, sh.nm.n_cand, lane);
+    if (warp == 0) {
+      pk_poses_of_candidates(sh, sh.nm.n_cand, lane);
+      if constexpr (DELTA) pk_delta_rows(sh, sh.nm.n_cand, lane);
+    }
     if (t == 0) sh.n_poses = sh.nm.n_cand;
   } else {
     const int pc = min(a.chunk, a.n_total);
-    if (t < pc) pk_pose_from_list(sh, t, a.poses_in + 12 * static_cast<size_t>(t));
+    if (t < pc) pk_pose_from_list(sh, t, a.poses_in + 12 * static_cast<size_t>(t));  // pc <= 8: warp 0
+    if (DELTA && warp == 0) pk_delta_rows(sh, pc, lane);
     if (t == 0) sh.n_poses = pc;
   }
   for (int i = t; i < PK_MAX_POSES * 2 * PK_MAX_BINS; i += PK_THREADS) (&sh.bmarg[0][0])[i] = 0;
@@ -1183,6 +1256,7 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
     // rotates three (every block reads all of them; buffer b is zeroed while batch b + 1 is finalized, see (B))
     const int buf = solve_mode ? static_cast<int>(batch % 3ull) : static_cast<int>(batch & 1ull);
     if (blockIdx.x == 0 && t == 0) pk_stamp(a, batch, 0);
+    if (DELTA && blockIdx.x == 0 && t == 0 && sh.delta_on && a.delta_stats) a.delta_stats[0] += 1ull, a.delta_stats[1] += static_cast<unsigned long long>(n_poses);
     // pose-list mode runs ahead of the finalizers: buffer `buf` (accumulators, tile counter) must have been finalized for
     // chunk batch - 2 first.  (Nelder-Mead mode: seeing the scores of batch - 1 already implies it.)
     if (!solve_mode && batch >= 2) {
@@ -1251,7 +1325,7 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
           const unsigned int refill = rs.w == 0u ? PK_RING - 1u : rs.w - 1u;
           pk_ring_fill<K>(pk_ring_slot<K>(a, smem_base, refill), B.points + static_cast<size_t>(rs.x + (PK_RING - 1) * rs.z) * TP + lane, rs.y > PK_RING - 1u);
           sts_v4(ring_state, make_uint4(rs.x + rs.z, rs.y - 1u, rs.z, rs.w + 1u == PK_RING ? 0u : rs.w + 1u));
-          pk_tile<MODEL, K, false, ATOM, TMA>(a, sh, B, n_poses, w, rs.x * TP, bag_n, q);
+          pk_tile<MODEL, K, false, ATOM, TMA, DPOSE>(a, sh, B, n_poses, w, rs.x * TP, bag_n, q);
         }
         // the cloud's ragged last tile (fewer than 32 * K points, register loads) belongs to the warp whose tile sequence reaches it
         const unsigned int n_full = bag_n / TP;
@@ -1361,6 +1435,7 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
       const int pc = static_cast<int>(max(0ll, min(static_cast<long long>(a.chunk), static_cast<long long>(a.n_total) - next0)));
       __syncthreads();
       if (t < pc) pk_pose_from_list(sh, t, a.poses_in + 12 * static_cast<size_t>(next0 + t));
+      if (DELTA && warp == 0) pk_delta_rows(sh, pc, lane);
       if (t == 0) sh.n_poses = pc;
       __syncthreads();
       continue;
@@ -1472,6 +1547,7 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
       }
       const int n_next = sh.nm.n_cand;  // 0 when finished
       pk_poses_of_candidates(sh, n_next, lane);
+      if constexpr (DELTA) pk_delta_rows(sh, n_next, lane);
       if (lane == 0) {
         sh.n_poses = n_next;
         sh.tmax = pk_tmax(sh, n_next);
@@ -1486,6 +1562,10 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
     if (blockIdx.x == 0 && t == 0) pk_stamp(a, batch, 6);
   }
 
+  if (a.delta_stats && lane == 0) {
+    atomicAdd(a.delta_stats + 2, static_cast<unsigned long long>(sh.deferred[warp][0]));
+    atomicAdd(a.delta_stats + 3, static_cast<unsigned long long>(sh.deferred[warp][1]));
+  }
   if constexpr (TMA) {
     if (a.tma_stats) {
       const unsigned int nw = __reduce_add_sync(0xffffffffu, w.n_window), ne = __reduce_add_sync(0xffffffffu, w.n_escaped);
@@ -1517,13 +1597,18 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
 
 // debug / test kernel: the lean classifier AND the exact path on every (point, pose); a.dbg: [0] point-poses,
 // [1] verdicts deferred to the exact path, [2] kept verdicts that disagree with the exact path (must be 0),
-// [3] max over accepted verdicts of |uv_fp32 - uv_exact| / E as float bits (atomicMax; must stay < 1)
-template <int MODEL>
+// [3] max over accepted verdicts of |uv_fp32 - uv_exact| / E as float bits (atomicMax; must stay < 1).
+// DELTA (equirectangular, packed): pose 0 through the anchor step, poses 1..n-1 through the delta step of the hot loop.
+template <int MODEL, bool DELTA = false>
 __global__ void __launch_bounds__(NID_THREADS) nid_lean_verify_kernel(const __grid_constant__ NidArgs a, const __grid_constant__ LeanCam lc) {
   const float4* __restrict__ pts = static_cast<const float4*>(a.points);
   unsigned long long total = 0, uncertain = 0, mismatch = 0;
   float tmax = 0.f, max_ratio = 0.f;
   for (int p = 0; p < a.n_poses; p++) tmax = fmaxf(tmax, a.pose32[p][12]);
+  float Q[NID_MAX_POSES][16];
+  if constexpr (DELTA) {
+    for (int p = 1; p < a.n_poses; p++) lean_delta_pose(a.pose[p], a.pose[0], Q[p]);
+  }
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
   // points in pairs (2k, 2k + 1), as the hot loop classifies them when the packed classifier is compiled in
   for (long long k = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; 2 * k < a.n; k += stride) {
@@ -1532,9 +1617,17 @@ __global__ void __launch_bounds__(NID_THREADS) nid_lean_verify_kernel(const __gr
     const float4 q2[2] = {__ldg(pts + i0), __ldg(pts + i1)};
     float delta[2];
     for (int h = 0; h < 2; h++) delta[h] = (5.25f * F32_U) * (fabsf(q2[h].x) + fabsf(q2[h].y) + fabsf(q2[h].z) + tmax);
+    LeanAnchor2 an;
     for (int p = 0; p < a.n_poses; p++) {
       LeanVerdict v2[2];
-      if constexpr (PK_PACKED_FP32 && LeanPacked<MODEL>::value) {
+      if constexpr (DELTA) {
+        const F2 X = f2_pack(q2[0].x, q2[1].x), Y = f2_pack(q2[0].y, q2[1].y), Z = f2_pack(q2[0].z, q2[1].z), D = f2_pack(delta[0], delta[1]);
+        const LeanVerdict2 w = p == 0 ? classify_lean2_anchor<MODEL>(a.fast, lc, a.width, a.pose32[0], X, Y, Z, D, an) : classify_lean2_delta<MODEL>(lc, a.width, Q[p], X, Y, Z, D, an);
+        for (int h = 0; h < 2; h++) {
+          v2[h].accept = w.accept[h], v2[h].uncertain = w.uncertain[h], v2[h].idx = w.idx[h];
+          v2[h].up = w.up[h], v2[h].vp = w.vp[h], v2[h].hx = w.hx[h], v2[h].hy = w.hy[h];
+        }
+      } else if constexpr (PK_PACKED_FP32 && LeanPacked<MODEL>::value) {
         const LeanVerdict2 w = classify_lean2<MODEL>(a.fast, lc, a.width, a.pose32[p], f2_pack(q2[0].x, q2[1].x), f2_pack(q2[0].y, q2[1].y),
                                                      f2_pack(q2[0].z, q2[1].z), f2_pack(delta[0], delta[1]));
         for (int h = 0; h < 2; h++) {
