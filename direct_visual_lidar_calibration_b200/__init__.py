@@ -11,6 +11,7 @@ this package is the thin host-side mirror of the reference's interface for that 
   NelderMead                    <- dfo::NelderMead<N>                (include/dfo/nelder_mead.hpp)
   VisualCameraCalibrationParams, VisualCameraCalibration <- vlcal::VisualCameraCalibration
                                                                      (include/vlcal/calib/visual_camera_calibration.hpp)
+  PoseEstimationParams, PoseEstimation <- vlcal::PoseEstimation      (include/vlcal/common/estimate_pose.hpp)
 
 There is no CPU fallback: without the built library or without a CUDA device every compute call raises.
 """
@@ -21,6 +22,7 @@ from .culling import ViewCulling, ViewCullingParams, generate_lidar_image
 from .nelder_mead import NelderMead, NelderMeadParams
 from . import bfgs
 from .calibration import RegistrationType, VisualCameraCalibration, VisualCameraCalibrationParams, estimate_camera_fov, se3_expmap
+from .pose_estimation import PoseEstimation, PoseEstimationParams
 
 __all__ = [
     "score_poses",
@@ -31,4 +33,5 @@ __all__ = [
     "ViewCulling", "ViewCullingParams",
     "NelderMead", "NelderMeadParams",
     "RegistrationType", "VisualCameraCalibration", "VisualCameraCalibrationParams", "estimate_camera_fov", "se3_expmap",
+    "PoseEstimation", "PoseEstimationParams",
 ]

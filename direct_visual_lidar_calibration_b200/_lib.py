@@ -96,6 +96,17 @@ class BfgsResult(C.Structure):
     ]
 
 
+class PoseEstimationParams(C.Structure):
+    _fields_ = [("ransac_iterations", C.c_int), ("ransac_error_thresh", C.c_double), ("robust_kernel_width", C.c_double)]
+
+
+class PoseEstimationStats(C.Structure):
+    _fields_ = [
+        ("hypotheses", C.c_int), ("degenerate", C.c_int), ("best_index", C.c_int), ("best_inliers", C.c_int),
+        ("lm_iterations", C.c_int), ("final_cost", C.c_double),
+    ]
+
+
 SE3_OBJECTIVE = C.CFUNCTYPE(C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_void_p)
 NM_BATCH_FN = C.CFUNCTYPE(None, C.POINTER(C.c_double), C.c_int, C.c_int, C.POINTER(C.c_double), C.c_void_p)
 NM_OBSERVE_FN = C.CFUNCTYPE(None, C.POINTER(C.c_double), C.c_int, C.c_double, C.c_void_p)
@@ -175,6 +186,14 @@ def load_library():
     L.vlcal_bfgs_default_params.restype = None
     L.vlcal_bfgs_minimize_se3.argtypes = [SE3_OBJECTIVE, vp, C.POINTER(BfgsParams), dp, POSE_CALLBACK, vp, dp, C.POINTER(BfgsResult)]
     L.vlcal_estimate_pose_bfgs_ctx.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(BfgsParams), dp, POSE_CALLBACK, ALLREDUCE_FN, vp, dp, C.POINTER(BfgsResult)]
+    L.vlcal_pose_estimation_default_params.argtypes = [C.POINTER(PoseEstimationParams)]
+    L.vlcal_pose_estimation_default_params.restype = None
+    cam = [C.c_int, dp, C.c_int, dp, C.c_int]
+    L.vlcal_estimate_pose_from_correspondences.argtypes = [C.c_int] + cam + [dp, dp, C.c_int64, C.POINTER(PoseEstimationParams), dp, vp, C.POINTER(PoseEstimationStats)]
+    L.vlcal_estimate_directions.argtypes = cam + [dp, C.c_int64, dp]
+    L.vlcal_pose_debug_score_pairs.argtypes = [C.c_int] + cam + [dp, dp, C.c_int64, vp, C.c_int, C.c_double, vp, vp, dp]
+    L.vlcal_pose_debug_sample_pairs.argtypes = [C.c_int64, C.c_int, vp]
+    L.vlcal_pose_debug_refine.argtypes = cam + [dp, dp, C.c_int64, C.c_double, dp, dp, ip, dp]
     _lib = L
     return L
 

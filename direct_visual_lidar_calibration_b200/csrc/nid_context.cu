@@ -87,28 +87,31 @@ static void fov_to_dir(const double x[2], double dir[3]) {
   for (int i = 0; i < 3; i++) dir[i] = v[i] + qw * uv[i] + c[i];
 }
 
+void estimate_direction_host(const CameraParams& cam, const double target[2], double dir[3]) {
+  auto f = [&](const double* xs, int count, double* ys) {  // estimate_fov.cpp:22-26
+    for (int i = 0; i < count; i++) {
+      double d[3], u, v;
+      fov_to_dir(xs + 2 * i, d);
+      project_exact_dyn(cam, d[0], d[1], d[2], &u, &v);
+      const double ex = target[0] - u, ey = target[1] - v;
+      const double err = ex * ex + ey * ey;
+      ys[i] = std::isfinite(err) ? err : DBL_MAX;
+    }
+  };
+  auto observe = [](const double*, double) {};
+  const double x0[2] = {0.0, 0.0};
+  host::NelderMeadParams p;  // :29 defaults
+  const host::NelderMeadResult r = host::nelder_mead(2, f, observe, x0, p, /*speculate=*/false);
+  fov_to_dir(r.x.data(), dir);  // :33
+}
+
 double estimate_camera_fov_host(const CameraParams& cam, int width, int height) {
   // estimate_fov.cpp:37 (integer divisions), :39-48
   const double corners[3][2] = {{0.0, 0.0}, {static_cast<double>(width / 2), 0.0}, {0.0, static_cast<double>(height / 2)}};
   double max_fov = 0.0;
   for (int k = 0; k < 3; k++) {
-    const double* target = corners[k];
-    auto f = [&](const double* xs, int count, double* ys) {  // :22-26
-      for (int i = 0; i < count; i++) {
-        double dir[3], u, v;
-        fov_to_dir(xs + 2 * i, dir);
-        project_exact_dyn(cam, dir[0], dir[1], dir[2], &u, &v);
-        const double ex = target[0] - u, ey = target[1] - v;
-        const double err = ex * ex + ey * ey;
-        ys[i] = std::isfinite(err) ? err : DBL_MAX;
-      }
-    };
-    auto observe = [](const double*, double) {};
-    const double x0[2] = {0.0, 0.0};
-    host::NelderMeadParams p;  // :29 defaults
-    const host::NelderMeadResult r = host::nelder_mead(2, f, observe, x0, p, /*speculate=*/false);
     double dir[3];
-    fov_to_dir(r.x.data(), dir);  // :33
+    estimate_direction_host(cam, corners[k], dir);
     const double n2 = (dir[0] * dir[0] + dir[1] * dir[1]) + dir[2] * dir[2];
     const double nz = n2 > 0.0 ? dir[2] / std::sqrt(n2) : dir[2];
     const double fov = std::acos(nz);  // :43

@@ -26,6 +26,8 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line);
 
 // validated camera (create_camera.cpp:17-32 rules)
 int make_camera(int model, const double* intr, int n_intr, const double* dist, int n_dist, CameraParams* out);
+// estimate_direction (estimate_fov.cpp:17-34): the bearing whose projection is nearest pixel `target`, by NelderMead<2>
+void estimate_direction_host(const CameraParams& cam, const double target[2], double dir[3]);
 // estimate_camera_fov (estimate_fov.cpp:36-51)
 double estimate_camera_fov_host(const CameraParams& cam, int width, int height);
 

@@ -6,6 +6,8 @@
   <data_path>/calib.json  camera.{camera_model,intrinsics,distortion_coeffs}, meta.bag_names,
                           results.{init_T_lidar_camera[_auto], T_lidar_camera} = [x y z qx qy qz qw] of T_lidar_camera
                           (preprocess.cpp:220-232, calibrate.cpp:38-45,57-76,128-140)
+  <data_path>/<bag>_lidar_indices.png  int32 point-index map of the LiDAR image as 8UC4  (preprocess.cpp:205-211)
+  <data_path>/<bag>_matches.json       kpts0 / kpts1 / matches / confidence  (find_matches_superglue.py:115-117)
 The PLY writer/reader of the reference is Iridescence's glk::save_ply_binary / glk::load_ply (not vendored); the reader here
 parses the header generically (binary little endian or ascii, any property order, float/double/int types)."""
 from __future__ import annotations
@@ -102,6 +104,89 @@ def load_visual_lidar_data(data_path: str, bag_name: str):
     if inten is None:
         raise ValueError(f"{bag_name}.ply has no intensity property")
     return VisualLiDARData(image, pts, inten)
+
+
+def save_lidar_indices(path: str, index_image) -> None:
+    """<bag>_lidar_indices.png: the int32 point-index map (-1 = no point) written as an 8UC4 PNG, the way preprocess does
+    (preprocess.cpp:207-211).  cv2 swaps B and R on write and back on read, so the bytes round-trip exactly."""
+    import cv2
+
+    idx = np.ascontiguousarray(np.asarray(index_image, dtype="<i4"))
+    if idx.ndim != 2:
+        raise ValueError("index image must be H x W")
+    if not cv2.imwrite(path, idx.view(np.uint8).reshape(idx.shape[0], idx.shape[1], 4)):
+        raise OSError(f"failed to write {path}")
+
+
+def load_lidar_indices(path: str) -> np.ndarray:
+    """cv::imread(path, -1) reinterpreted as CV_32SC1 (initial_guess_auto.cpp:82-83) -> int32 (H, W)."""
+    import cv2
+
+    img = cv2.imread(path, cv2.IMREAD_UNCHANGED)
+    if img is None:
+        raise FileNotFoundError(f"failed to load {path}")
+    if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 4:
+        raise ValueError(f"{path}: expected an 8-bit 4-channel PNG (the int32 point-index map), got {img.dtype} {img.shape}")
+    return np.ascontiguousarray(img).view("<i4").reshape(img.shape[0], img.shape[1]).astype(np.int32)
+
+
+def _json_ints(values, name: str) -> np.ndarray:
+    """std::vector<int> from a JSON number array: nlohmann converts each number with static_cast<int> (truncation)."""
+    a = np.trunc(np.asarray(values, dtype=np.float64).reshape(-1))
+    if not np.all(np.isfinite(a)) or np.any(np.abs(a) > 2**31 - 1):
+        raise ValueError(f"{name}: values must be finite and fit in int32")
+    return a.astype(np.int64)
+
+
+def load_matches(path: str) -> dict:
+    """<bag>_matches.json of find_matches_superglue.py (:115-117): flat kpts0 / kpts1 lists of x, y pairs, matches (index into
+    kpts1 or -1 per kpts0 entry), confidence.  Keypoints and matches come back as the reference reads them: truncated ints."""
+    with open(path) as f:
+        m = json.load(f)
+    kpts0, kpts1, matches = (_json_ints(m[k], k) for k in ("kpts0", "kpts1", "matches"))
+    if kpts0.size % 2 or kpts1.size % 2 or matches.size != kpts0.size // 2:
+        raise ValueError(f"{path}: kpts0 / kpts1 must hold x, y pairs and matches one entry per kpts0 keypoint")
+    return {"kpts0": kpts0.reshape(-1, 2), "kpts1": kpts1.reshape(-1, 2), "matches": matches, "confidence": np.asarray(m.get("confidence", []), dtype=np.float64)}
+
+
+# the 8 neighbours of a keypoint, nearest first (initial_guess_auto.cpp:35-43)
+_PICK_OFFSETS = [(dx, dy) for dx in (-1, 0, 1) for dy in (-1, 0, 1) if (dx, dy) != (0, 0)]
+_PICK_OFFSETS.sort(key=lambda o: o[0] * o[0] + o[1] * o[1])
+
+
+def read_correspondences(data_path: str, bag_name: str, points):
+    """InitialGuessAuto::read_correspondences (initial_guess_auto.cpp:81-125) -> (kp0 float64 (K,2), points float64 (K,3)).
+
+    A match is used when matches[i] >= 0 and the LiDAR-image keypoint kpts1[matches[i]] lies on a pixel with a point; the 3-D
+    point is points[index] of the bag's full cloud, the 2-D point the truncated camera keypoint.  Where the pixel is blank the
+    reference searches the 8 neighbours but then skips the match whatever it found (the found index is never used); that
+    behaviour is kept on purpose, so results match the reference's, with its warning when no neighbour has a point either.
+    Unlike the reference, a kpts1 keypoint outside the index image, a match index past kpts1 or a point index past the cloud
+    is an error instead of an out-of-bounds read."""
+    pts = np.asarray(points, dtype=np.float64)
+    index_image = load_lidar_indices(os.path.join(data_path, bag_name + "_lidar_indices.png"))
+    m = load_matches(os.path.join(data_path, bag_name + "_matches.json"))
+    H, W = index_image.shape
+    kp0_out, pt_out = [], []
+    for i, match in enumerate(m["matches"]):
+        if match < 0:
+            continue
+        if match >= m["kpts1"].shape[0]:
+            raise ValueError(f"{bag_name}_matches.json: matches[{i}] = {match} is past the {m['kpts1'].shape[0]} kpts1 keypoints")
+        x, y = (int(v) for v in m["kpts1"][match])
+        if not (0 <= x < W and 0 <= y < H):
+            raise ValueError(f"{bag_name}_matches.json: kpts1[{match}] = ({x}, {y}) is outside the {W}x{H} LiDAR index image")
+        index = int(index_image[y, x])
+        if index < 0:
+            found = any(0 <= x + dx < W and 0 <= y + dy < H and index_image[y + dy, x + dx] >= 0 for dx, dy in _PICK_OFFSETS)
+            if not found:
+                print("warning: ignore keypoint in a blank region!!")
+            continue
+        if index >= pts.shape[0]:
+            raise ValueError(f"{bag_name}_lidar_indices.png: point index {index} at ({x}, {y}) is past the {pts.shape[0]} points of {bag_name}.ply")
+        kp0_out.append(m["kpts0"][i].astype(np.float64))
+        pt_out.append(pts[index, :3])
+    return np.array(kp0_out, dtype=np.float64).reshape(-1, 2), np.array(pt_out, dtype=np.float64).reshape(-1, 3)
 
 
 def load_calib_json(data_path: str) -> dict:

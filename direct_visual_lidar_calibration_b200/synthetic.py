@@ -271,3 +271,105 @@ def pose_grid(T_center: np.ndarray, n_rot=(8, 8, 8), n_trans=(2, 4, 4), rot_half
                         for tz in axes_t[2]:
                             out.append(perturb(T_center, (rx, ry, rz), (tx, ty, tz)))
     return np.stack(out)
+
+
+# ---------------------------------------------------------------------------------------------
+# initial_guess_auto datasets
+# ---------------------------------------------------------------------------------------------
+
+def _axis_rotation(axis: int, angle: float) -> np.ndarray:
+    c, s = math.cos(angle), math.sin(angle)
+    i, j = (axis + 1) % 3, (axis + 2) % 3
+    R = np.eye(3)
+    R[i, i], R[i, j], R[j, i], R[j, j] = c, -s, s, c
+    return R
+
+
+def virtual_lidar_camera(lidar_fov: float):
+    """The virtual camera preprocess renders the LiDAR image with (preprocess.cpp:180-197): below a 150 deg LiDAR FoV a
+    1024 x 1024 pinhole looking along LiDAR +x, otherwise a 1920 x 960 equirectangular image.
+    -> (camera_model, intrinsics, (W, H), T_camera_lidar of the virtual camera)."""
+    T_lidar_camera = np.eye(4)
+    if lidar_fov < math.radians(150.0):
+        W, H = 1024, 1024
+        T_lidar_camera[:3, :3] = _axis_rotation(1, math.pi / 2) @ _axis_rotation(2, -math.pi / 2)
+        fx = W / (2.0 * math.tan(lidar_fov / 2.0))
+        model, intr = "plumb_bob", [fx, fx, W / 2.0, H / 2.0]
+    else:
+        W, H = 1920, 960
+        T_lidar_camera[:3, :3] = _axis_rotation(0, -math.pi / 2)
+        model, intr = "equirectangular", [float(W), float(H)]
+    T_camera_lidar = np.eye(4)
+    T_camera_lidar[:3, :3] = T_lidar_camera[:3, :3].T
+    return model, intr, (W, H), T_camera_lidar
+
+
+def write_initial_guess_dataset(
+    data_path: str, n_bags: int = 2, camera_key: str = "pinhole_640x480", pattern: str = "frustum", n_points: int = 30_000, n_matches: int = 300,
+    outlier_fraction: float = 0.25, unmatched_fraction: float = 0.1, blank_fraction: float = 0.05, lidar_fov_deg: float = 120.0, seed: int = 0, device: int = -1):
+    """A preprocessed dataset as initial_guess_auto finds it: calib.json (camera + meta.bag_names, no results), and per bag
+    <bag>.png, <bag>.ply, <bag>_lidar_indices.png (generate_lidar_image through the virtual LiDAR camera, on the GPU) and
+    <bag>_matches.json.  Matches pair a LiDAR-image pixel (float keypoint inside it) with the ground-truth projection of its
+    point into the camera (float keypoint); `outlier_fraction` of the matches get a random camera keypoint instead, and the
+    file also holds unmatched keypoints (match -1) and matches onto blank LiDAR-image pixels.  Returns the bags (make_bag
+    dicts) with the ground truth T_gt (T_camera_lidar)."""
+    import json
+    import os
+
+    import cv2
+
+    from . import io as vio
+    from .camera import create_camera
+    from .culling import generate_lidar_image
+
+    rng = np.random.default_rng(seed)
+    vmodel, vintr, vsize, T_vcam_lidar = virtual_lidar_camera(math.radians(lidar_fov_deg))
+    vproj = create_camera(vmodel, vintr, [])
+    bags, names = [], []
+    for b in range(n_bags):
+        bag = make_bag(camera_key, pattern, n_points, config_index=7, bag_index=b)
+        name = f"bag{b}"
+        cv2.imwrite(os.path.join(data_path, name + ".png"), bag["image"])
+        vio.save_ply_binary(os.path.join(data_path, name + ".ply"), bag["points"][:, :3], bag["intensities"])
+        _, index_image = generate_lidar_image(vproj, vsize, T_vcam_lidar, bag["points"], bag["intensities"], device=device)
+        vio.save_lidar_indices(os.path.join(data_path, name + "_lidar_indices.png"), index_image)
+
+        # LiDAR-image pixels whose point lands in front of the camera, inside the image
+        proj = create_camera(bag["camera_model"], bag["intrinsics"], bag["distortion"])
+        ys, xs = np.nonzero(index_image >= 0)
+        pick = rng.permutation(xs.size)[: 4 * n_matches]
+        xs, ys = xs[pick], ys[pick]
+        pc = bag["points"][index_image[ys, xs], :3] @ bag["T_gt"][:3, :3].T + bag["T_gt"][:3, 3]
+        uv = proj.project(pc)
+        ok = (pc[:, 2] > 0.1) & (uv[:, 0] >= 0) & (uv[:, 0] < bag["width"]) & (uv[:, 1] >= 0) & (uv[:, 1] < bag["height"])
+        xs, ys, uv = xs[ok][:n_matches], ys[ok][:n_matches], uv[ok][:n_matches]
+        n = xs.size
+        n_out = int(round(outlier_fraction * n))
+        uv[:n_out] = rng.uniform([0.0, 0.0], [bag["width"], bag["height"]], (n_out, 2))  # wrong matches
+        kpts1 = np.stack([xs, ys], axis=1) + rng.uniform(0.0, 0.999, (n, 2))
+        kpts0 = uv
+        matches = np.arange(n)
+        # matches onto blank LiDAR-image pixels, and unmatched keypoints
+        by, bx = np.nonzero(index_image < 0)
+        n_blank = int(round(blank_fraction * n))
+        pick = rng.choice(bx.size, n_blank, replace=False)
+        kpts1 = np.concatenate([kpts1, np.stack([bx[pick], by[pick]], axis=1) + 0.5])
+        kpts0 = np.concatenate([kpts0, rng.uniform([0.0, 0.0], [bag["width"], bag["height"]], (n_blank, 2))])
+        matches = np.concatenate([matches, n + np.arange(n_blank)])
+        n_unmatched = int(round(unmatched_fraction * n))
+        kpts0 = np.concatenate([kpts0, rng.uniform([0.0, 0.0], [bag["width"], bag["height"]], (n_unmatched, 2))])
+        matches = np.concatenate([matches, -np.ones(n_unmatched, dtype=np.int64)])
+        order = rng.permutation(matches.size)
+        result = {
+            "kpts0": kpts0[order].reshape(-1).tolist(), "kpts1": kpts1.reshape(-1).tolist(),
+            "matches": [int(v) for v in matches[order]], "confidence": rng.uniform(0.2, 1.0, matches.size).tolist(),
+        }
+        with open(os.path.join(data_path, name + "_matches.json"), "w") as f:
+            json.dump(result, f)
+        bag["n_outliers"] = n_out
+        bags.append(bag)
+        names.append(name)
+    model, intr, dist = bags[0]["camera_model"], bags[0]["intrinsics"], bags[0]["distortion"]
+    config = {"camera": {"camera_model": model, "intrinsics": list(intr), "distortion_coeffs": list(dist)}, "meta": {"bag_names": names}}
+    vio.save_calib_json(data_path, config)
+    return bags

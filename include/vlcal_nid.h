@@ -480,6 +480,96 @@ int vlcal_estimate_pose_bfgs_ctx(
   double T_out[16],
   vlcal_bfgs_result* result);
 
+/* ---- initial guess from 2D-3D correspondences: PoseEstimation (src/vlcal/common/estimate_pose.cpp) ------------------
+ * initial_guess_auto's solver.  1. bearings: camera side estimate_direction(kp0) (host NelderMead<2>, as
+ * estimate_camera_fov), LiDAR side the normalised point.  2. rotation RANSAC: hypotheses drawn on the host exactly as a
+ * one-thread reference run draws them (std::mt19937 seeded with mt19937()(), two uniform_int_distribution(0, M-1) draws per
+ * iteration); ONE kernel launch computes every hypothesis's rotation (Umeyama on its two bearing pairs) and counts the
+ * correspondences with |kp0 - project(R d_lidar)|^2 < ransac_error_thresh^2 (project_exact, never-contracted doubles).
+ * The winner is the largest count, ties to the lowest index; a second launch writes its inlier mask.  Hypotheses whose
+ * rotation is not unique (the same index twice, or bearings within 1e-9 of parallel / antiparallel on either side) score
+ * 0 and are counted in stats->degenerate.  3. refinement: Levenberg-Marquardt on SE(3) of
+ * 1/2 sum_i rho(|project(T p_i) - kp0_i|^2) over ALL correspondences, rho = Cauchy with b = robust_kernel_width^2, from
+ * [R_ransac | 0], with Ceres' default stopping rules (host; M is small).
+ * Errors: M < 2 (VLCAL_ERR_INVALID_ARGUMENT), no hypothesis with an inlier (VLCAL_ERR_INVALID_ARGUMENT). */
+typedef struct {
+  int ransac_iterations;      /* 8192 */
+  double ransac_error_thresh; /* 5.0 px */
+  double robust_kernel_width; /* 10.0 px */
+} vlcal_pose_estimation_params;
+
+typedef struct {
+  int hypotheses;   /* = ransac_iterations */
+  int degenerate;   /* hypotheses without a unique rotation (scored 0) */
+  int best_index;   /* winning hypothesis */
+  int best_inliers; /* its count */
+  int lm_iterations;
+  double final_cost; /* 1/2 sum rho(s_i) at T_camera_lidar_out */
+} vlcal_pose_estimation_stats;
+
+void vlcal_pose_estimation_default_params(vlcal_pose_estimation_params* p);
+
+/* kp0: M x 2 pixels, points: M x 3 (LiDAR frame).  T_camera_lidar_out: 4x4 column-major.  inlier_mask_out (optional):
+ * M bytes, 1 where the RANSAC winner's rotation reprojects the correspondence within the threshold.  device = -1: the
+ * current device. */
+int vlcal_estimate_pose_from_correspondences(
+  int device,
+  int camera_model,
+  const double* intrinsics,
+  int n_intrinsics,
+  const double* distortion,
+  int n_distortion,
+  const double* kp0,
+  const double* points,
+  int64_t n_correspondences,
+  const vlcal_pose_estimation_params* params,
+  double T_camera_lidar_out[16],
+  uint8_t* inlier_mask_out,
+  vlcal_pose_estimation_stats* stats_out);
+
+/* estimate_direction for n pixels (n x 2) -> n x 3 unit bearings (host) */
+int vlcal_estimate_directions(
+  int camera_model, const double* intrinsics, int n_intrinsics, const double* distortion, int n_distortion, const double* pixels, int64_t n, double* dirs_out);
+
+/* test hook: the RANSAC scoring launch on caller-given index pairs (n_pairs x 2, each in [0, M)).  counts_out: n_pairs
+ * int32 inlier counts; degenerate_out (optional): n_pairs bytes, 1 for a hypothesis without a unique rotation;
+ * kernel_ms_out (optional): the scoring launch's time between CUDA events. */
+int vlcal_pose_debug_score_pairs(
+  int device,
+  int camera_model,
+  const double* intrinsics,
+  int n_intrinsics,
+  const double* distortion,
+  int n_distortion,
+  const double* kp0,
+  const double* points,
+  int64_t n_correspondences,
+  const int32_t* pairs,
+  int n_pairs,
+  double ransac_error_thresh,
+  int32_t* counts_out,
+  uint8_t* degenerate_out,
+  double* kernel_ms_out);
+
+/* test hook: the index pairs the RANSAC draws for M correspondences (n_iterations x 2) */
+int vlcal_pose_debug_sample_pairs(int64_t n_correspondences, int n_iterations, int32_t* pairs_out);
+
+/* test hook: the Levenberg-Marquardt refinement alone from init_T_camera_lidar (column-major) */
+int vlcal_pose_debug_refine(
+  int camera_model,
+  const double* intrinsics,
+  int n_intrinsics,
+  const double* distortion,
+  int n_distortion,
+  const double* kp0,
+  const double* points,
+  int64_t n_correspondences,
+  double robust_kernel_width,
+  const double init_T_camera_lidar[16],
+  double T_camera_lidar_out[16],
+  int* iterations_out,
+  double* final_cost_out);
+
 #ifdef __cplusplus
 }
 #endif
