@@ -1,6 +1,8 @@
 // nid_bspline.cu -- host side of mode B: vlcal_nid_evaluate_bspline (reference: NIDCost::operator()<double>,
 // include/vlcal/costs/nid_cost.hpp:36-107; constructed per bag at visual_camera_calibration.cpp:203-206).
 #include <algorithm>
+#include <climits>
+#include <cmath>
 #include <cstring>
 
 #include "mem_pool.hpp"
@@ -47,6 +49,15 @@ static NidGKernel pick_g_kernel(int model, bool f32) {
   }
 }
 
+// hist_points and the inlier total are int counters (as in mode A)
+static int check_bspline_cloud(const vlcal_nid_ctx* ctx) {
+  if (ctx->cloud->n > INT_MAX) {
+    set_last_error("mode B counts inliers in 32-bit integers: clouds are limited to 2^31 - 1 points");
+    return VLCAL_ERR_UNSUPPORTED;
+  }
+  return VLCAL_OK;
+}
+
 struct PoolBuf {
   void* p = nullptr;
   int device = 0;
@@ -80,7 +91,9 @@ extern "C" int vlcal_nid_evaluate_bspline(vlcal_nid_ctx* ctx, const double* T_pa
     return VLCAL_ERR_INVALID_ARGUMENT;
   }
   VL_CUDA(cudaSetDevice(ctx->device));
+  if (const int rc = check_bspline_cloud(ctx); rc != VLCAL_OK) return rc;
   const int bins = ctx->bins, nb = bins * bins;
+  const int fixed_bits = nidb_fixed_bits(ctx->cloud->n);
   {  // one pose's joint histogram (8 B per bin) + marginal must fit the shared memory K2 opts into
     constexpr size_t SMEM_OPT_IN_CHECK = 100 * 1024;
     if (static_cast<size_t>(nb) * 8 + static_cast<size_t>(bins) * 4 + 64 > SMEM_OPT_IN_CHECK) {
@@ -122,6 +135,8 @@ extern "C" int vlcal_nid_evaluate_bspline(vlcal_nid_ctx* ctx, const double* T_pa
     for (int p = 0; p < pc; p++) std::memcpy(a.pose[p], T_params + 7 * static_cast<size_t>(p0 + p), 7 * sizeof(double));
     for (int i = 0; i < 4; i++)
       for (int j = 0; j < 4; j++) a.C[i][j] = C6[i][j] / 6.0;  // :33 spline_coeffs /= 6.0
+    a.fixed_one = std::ldexp(1.0, fixed_bits);
+    a.inv_one = std::ldexp(1.0, -fixed_bits);
     a.gjoint = static_cast<unsigned long long*>(gjoint.p);
     a.gpoints = static_cast<int*>(gpoints.p);
     a.counter = static_cast<unsigned int*>(counter.p);
@@ -162,7 +177,9 @@ extern "C" int vlcal_nid_evaluate_bspline_grad(vlcal_nid_ctx* ctx, const double*
     return VLCAL_ERR_INVALID_ARGUMENT;
   }
   VL_CUDA(cudaSetDevice(ctx->device));
+  if (const int rc = check_bspline_cloud(ctx); rc != VLCAL_OK) return rc;
   const int bins = ctx->bins, nb = bins * bins;
+  const int fixed_bits = nidb_fixed_bits(ctx->cloud->n);
   const size_t smem = static_cast<size_t>(nb) * 8 * 8 + static_cast<size_t>(bins) * 4 + 16;
   if (smem > 200 * 1024) {
     set_last_error("bins too large for the gradient kernel's shared-memory histogram (bins <= 56)");
@@ -201,6 +218,8 @@ extern "C" int vlcal_nid_evaluate_bspline_grad(vlcal_nid_ctx* ctx, const double*
     std::memcpy(a.pose, T_params + 7 * static_cast<size_t>(p), 7 * sizeof(double));
     for (int i = 0; i < 4; i++)
       for (int j = 0; j < 4; j++) a.C[i][j] = C6[i][j] / 6.0;
+    a.fixed_one = std::ldexp(1.0, fixed_bits);
+    a.inv_one = std::ldexp(1.0, -fixed_bits);
     a.gjoint = static_cast<unsigned long long*>(gjoint.p);
     a.gpart = static_cast<double*>(gpart.p);
     a.gpoints = static_cast<int*>(gpoints.p);

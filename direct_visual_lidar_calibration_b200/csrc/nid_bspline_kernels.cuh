@@ -4,9 +4,14 @@
 // floor() knot, bounds, hist_points[bin]++ and a 4x4 cubic-B-spline footprint splatted into the joint / image
 // histograms with weights beta_x[i]*beta_y[j] (the image itself is never interpolated).  No FoV test on this path.
 // Geometry and weights use the exact double path (exact_math.cuh) in the reference's operation order.
-// Accumulation: the weights are non-negative and <= 1, so they are accumulated as 2^-40 fixed-point integers with
-// 64-bit integer atomics -- order independent, hence deterministic run to run, at a quantisation of 4.5e-13 per tap
-// (|dNID| ~ 1e-11 against the serial double sum; tests use 1e-9).
+// Accumulation: the weights are non-negative and <= 1, so they are accumulated as 2^-F fixed-point integers with
+// 64-bit integer atomics -- order independent, hence deterministic run to run.  Every tap is rounded once to the nearest
+// multiple of 2^-F, so a bin holding m taps is within m * 2^-(F+1) of the exact sum of the per-tap doubles.
+// Headroom: the 16 weights of one point sum to 1, so a joint bin, and an image-marginal row sum in the finalize, holds at
+// most n * 2^F (plus m/2 of rounding) for a cloud of n points.  nidb_fixed_bits(n) = min(40, 62 - ceil(log2 n)) keeps
+// that below 2^62 < 2^64: F = 40 (4.5e-13 per tap) up to n = 2^22 points, F = 37 (3.6e-12 per tap) at 17.8 M points,
+// F = 31 at the 2^31 - 1 point limit of the int hist_points counters.  tests/test_gpu_mode_b_edges.py pins every bin
+// against the exact (math.fsum) sum of the reference's taps under that bound.
 #pragma once
 
 #include <cstdint>
@@ -18,7 +23,14 @@ namespace vlcal {
 
 constexpr int NIDB_MAX_POSES = 8;
 constexpr int NIDB_THREADS = 256;
-constexpr double NIDB_FIXED_ONE = 1099511627776.0;  // 2^40
+constexpr int NIDB_MAX_FIXED_BITS = 40;
+
+// fixed-point fraction bits for a cloud of n points: n * 2^F stays <= 2^62 in every joint bin and image row sum
+static inline int nidb_fixed_bits(long long n) {
+  int lg = 0;  // ceil(log2(max(n, 1)))
+  while (lg < 62 && (1ll << lg) < n) lg++;
+  return lg > 62 - NIDB_MAX_FIXED_BITS ? 62 - lg : NIDB_MAX_FIXED_BITS;
+}
 
 struct NidBArgs {
   const void* points;        // float4[n] or double4[n]
@@ -31,6 +43,7 @@ struct NidBArgs {
   CameraParams cam;
   double pose[NIDB_MAX_POSES][8];  // qx qy qz qw tx ty tz (Sophus::SE3d storage, :38)
   double C[4][4];                  // spline_coeffs / 6.0  (:29-33)
+  double fixed_one, inv_one;       // 2^F and 2^-F, F = nidb_fixed_bits(n)
   unsigned long long* gjoint;      // [NIDB_MAX_POSES][nb] fixed-point joint histogram accumulators
   int* gpoints;                    // [NIDB_MAX_POSES][bins] hist_points accumulators
   unsigned int* counter;
@@ -57,7 +70,7 @@ static __device__ void nidb_finalize(const NidBArgs& a, unsigned long long* smem
     for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
     __syncwarp();
     const double sum = static_cast<double>(part);  // :86 sum = hist_points.sum()
-    const double inv_one = 1.0 / NIDB_FIXED_ONE;
+    const double inv_one = a.inv_one;
     double t_j = 0.0, t_i = 0.0, t_p = 0.0;  // :88-94
     for (int k = lane; k < a.nb; k += 32) {
       const double pr = (static_cast<double>(__ldcg(g + k)) * inv_one) / sum;
@@ -158,7 +171,7 @@ __global__ void __launch_bounds__(NIDB_THREADS) nid_bspline_kernel(const __grid_
           xx = xx > 0 ? xx : 0;
           xx = xx < a.width - 1 ? xx : a.width - 1;
           const xd w = bx[i2] * by[j];
-          const long long q = __double2ll_rn(w.v * NIDB_FIXED_ONE);
+          const long long q = __double2ll_rn(w.v * a.fixed_one);
           atomicAdd(&hj[__ldg(row + xx)], static_cast<unsigned long long>(q));  // hist(bin_image, bin_points) += w
         }
       }
@@ -194,7 +207,7 @@ __global__ void __launch_bounds__(NIDB_THREADS) nid_bspline_kernel(const __grid_
 //   (u, v), J = d(u, v)/d pc                                       (camera model over xj3 duals)
 //   U_k = J_u . d pc/d theta_k,  V_k = J_v . d pc/d theta_k        (k = 0..6)
 //   w_ij = bx_i(sx) by_j(sy),  d w_ij/d theta_k = bx'_i by_j U_k + bx_i by'_j V_k
-// The joint histogram carries 1 + 7 accumulators per bin: the weights as 2^-40 fixed point (deterministic, as in K2),
+// The joint histogram carries 1 + 7 accumulators per bin: the weights as 2^-F fixed point (deterministic, as in K2),
 // the partials as doubles (their range is unbounded; double atomics, so bits may differ run to run at the 1e-13 level).
 // The last block turns them into NID and d NID/d theta through the entropy chain rule.
 constexpr int NIDG_THREADS = 256;
@@ -208,6 +221,7 @@ struct NidGArgs {
   CameraParams cam;
   double pose[8];
   double C[4][4];
+  double fixed_one, inv_one;   // 2^F and 2^-F, F = nidb_fixed_bits(n)
   unsigned long long* gjoint;  // [nb] fixed-point weights
   double* gpart;               // [nb][7] partial sums
   int* gpoints;                // [bins]
@@ -323,12 +337,12 @@ __global__ void __launch_bounds__(NIDG_THREADS) nid_bspline_grad_kernel(const __
 #pragma unroll
       for (int t = 0; t < 4; t++) {
         if ((done >> t) & 1u) continue;
-        long long wq = __double2ll_rn(tw[t] * NIDB_FIXED_ONE);
+        long long wq = __double2ll_rn(tw[t] * a.fixed_one);
         double gx = tgx[t], gy = tgy[t];
 #pragma unroll
         for (int t2 = t + 1; t2 < 4; t2++) {
           if (tb[t2] == tb[t]) {
-            wq += __double2ll_rn(tw[t2] * NIDB_FIXED_ONE);
+            wq += __double2ll_rn(tw[t2] * a.fixed_one);
             gx += tgx[t2], gy += tgy[t2];
             done |= 1u << t2;
           }
@@ -366,7 +380,7 @@ __global__ void __launch_bounds__(NIDG_THREADS) nid_bspline_grad_kernel(const __
   __shared__ double s_red[NIDG_THREADS];
   __shared__ double s_sum;
   double* jv = reinterpret_cast<double*>(s_w);
-  const double inv_one = 1.0 / NIDB_FIXED_ONE;
+  const double inv_one = a.inv_one;
   int part = 0;
   for (int k = threadIdx.x; k < a.bins; k += blockDim.x) part += __ldcg(a.gpoints + k);
   s_red[threadIdx.x] = static_cast<double>(part);

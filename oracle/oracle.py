@@ -99,6 +99,8 @@ def lib():
         L.orc_create_camera.argtypes = [C.c_char_p, dp, C.c_int, dp, C.c_int, C.POINTER(Camera)]
         L.orc_create_camera.restype = C.c_int
         L.orc_project.argtypes = [C.POINTER(Camera), dp, dp]
+        L.orc_project_n.argtypes = [C.POINTER(Camera), dp, C.c_int64, dp]
+        L.orc_project_n.restype = None
         L.orc_se3_expmap_gtsam.argtypes = [dp, dp]
         L.orc_isometry_mul.argtypes = [dp, dp, dp]
         L.orc_isometry_inverse.argtypes = [dp, dp]
@@ -163,9 +165,7 @@ def create_camera(model: str, intrinsics, distortion):
 def project(cam: Camera, p) -> np.ndarray:
     pts = _f64(p).reshape(-1, 3)
     out = np.empty((pts.shape[0], 2))
-    L = lib()
-    for i in range(pts.shape[0]):
-        L.orc_project(C.byref(cam), _dp(pts[i]), _dp(out[i]))
+    lib().orc_project_n(C.byref(cam), _dp(pts), pts.shape[0], _dp(out))  # orc_project per point
     return out if np.asarray(p).ndim > 1 else out[0]
 
 

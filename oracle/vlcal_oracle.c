@@ -795,6 +795,10 @@ int64_t orc_view_cull(
   return count;
 }
 
+void orc_project_n(const orc_camera* cam, const double* p, int64_t n, double* uv) {
+  for (int64_t i = 0; i < n; i++) orc_project(cam, p + 3 * i, uv + 2 * i);
+}
+
 /* ------------------------------------------------------------------------------------------
  * NIDCost::operator()<double>   include/vlcal/costs/nid_cost.hpp:36-107  (mode B)
  * ---------------------------------------------------------------------------------------- */

@@ -58,6 +58,8 @@ int orc_create_camera(const char* camera_model, const double* intrinsics, int n_
 
 /* GenericCamera<Projection>::project  include/camera/generic_camera.hpp:21-28 */
 void orc_project(const orc_camera* cam, const double p[3], double uv[2]);
+/* orc_project over n points: p[3n] -> uv[2n] */
+void orc_project_n(const orc_camera* cam, const double* p, int64_t n, double* uv);
 
 /* gtsam::Pose3::Expmap(x).matrix(), x = (wx,wy,wz,vx,vy,vz); 4x4 column-major out.
  * call sites: src/vlcal/calib/visual_camera_calibration.cpp:104,129 */
