@@ -194,6 +194,11 @@ def load_library():
     L.vlcal_pose_debug_score_pairs.argtypes = [C.c_int] + cam + [dp, dp, C.c_int64, vp, C.c_int, C.c_double, vp, vp, dp]
     L.vlcal_pose_debug_sample_pairs.argtypes = [C.c_int64, C.c_int, vp]
     L.vlcal_pose_debug_refine.argtypes = cam + [dp, dp, C.c_int64, C.c_double, dp, dp, ip, dp]
+    i64p = C.POINTER(C.c_int64)
+    L.vlcal_approximate_voxel_grid.argtypes = [C.c_int, vp, C.c_int64, C.c_double, vp, i64p, i64p, dp]
+    L.vlcal_equalize_intensities.argtypes = [C.c_int, vp, C.c_int64, vp, dp]
+    L.vlcal_lidar_fov_candidates.argtypes = [C.c_int, vp, C.c_int64, vp, i64p, ip, dp]
+    L.vlcal_min_bearing_cosine.argtypes = [C.c_int, vp, C.c_int64, dp]
     _lib = L
     return L
 

@@ -85,6 +85,150 @@ def load_ply(path: str):
     return np.ascontiguousarray(pts), inten
 
 
+# PCD TYPE/SIZE -> numpy type
+_PCD_TYPES = {
+    ("I", "1"): "i1", ("I", "2"): "i2", ("I", "4"): "i4", ("I", "8"): "i8",
+    ("U", "1"): "u1", ("U", "2"): "u2", ("U", "4"): "u4", ("U", "8"): "u8",
+    ("F", "4"): "f4", ("F", "8"): "f8",
+}
+
+
+def _read_pcd_fields(path: str):
+    """PCD v0.7 (ascii or binary) -> [(name, numpy type, count, values (N, count))]."""
+    with open(path, "rb") as f:
+        head = {}
+        while True:
+            line = f.readline()
+            if not line:
+                raise ValueError(f"{path}: truncated PCD header")
+            tok = line.decode("ascii", errors="replace").split()
+            if not tok or tok[0].startswith("#"):
+                continue
+            head[tok[0].upper()] = tok[1:]
+            if tok[0].upper() == "DATA":
+                break
+        for key in ("FIELDS", "SIZE", "TYPE"):
+            if key not in head:
+                raise ValueError(f"{path}: PCD header has no {key} line")
+        names, sizes, types = head["FIELDS"], head["SIZE"], head["TYPE"]
+        counts = [int(c) for c in head.get("COUNT", ["1"] * len(names))]
+        if not (len(names) == len(sizes) == len(types) == len(counts)):
+            raise ValueError(f"{path}: PCD FIELDS / SIZE / TYPE / COUNT lengths differ")
+        if "POINTS" in head:
+            n = int(head["POINTS"][0])
+        else:
+            n = int(head.get("WIDTH", ["0"])[0]) * int(head.get("HEIGHT", ["1"])[0])
+        try:
+            dtypes = [_PCD_TYPES[(t.upper(), s)] for t, s in zip(types, sizes)]
+        except KeyError as e:
+            raise ValueError(f"{path}: unknown PCD field type {e.args[0]}") from None
+        data = head["DATA"][0].lower() if head["DATA"] else ""
+        if data == "binary_compressed":
+            raise ValueError(f"{path}: binary_compressed (LZF) PCD is not supported; save the map as binary or ascii PCD")
+        widths = [max(c, 1) for c in counts]
+        if data == "binary":
+            dt = np.dtype([(f"f{i}", "<" + t, (w,)) for i, (t, w) in enumerate(zip(dtypes, widths))])
+            raw = f.read(dt.itemsize * n)
+            if len(raw) < dt.itemsize * n:
+                raise ValueError(f"{path}: PCD data holds fewer than the {n} points its header declares")
+            rec = np.frombuffer(raw, dtype=dt, count=n)
+            cols = [rec[f"f{i}"].reshape(n, widths[i]) for i in range(len(names))]
+        elif data == "ascii":
+            total = sum(widths)
+            vals = np.loadtxt(f, dtype=np.float64, max_rows=n, ndmin=2) if n else np.zeros((0, total))
+            if vals.shape != (n, total):
+                raise ValueError(f"{path}: ascii PCD data is {vals.shape[0]} x {vals.shape[1]}, the header declares {n} x {total}")
+            cols, c0 = [], 0
+            for t, w in zip(dtypes, widths):
+                cols.append(vals[:, c0 : c0 + w].astype(t))
+                c0 += w
+        else:
+            raise ValueError(f"{path}: unknown PCD DATA kind {data!r}")
+    return [(nm, t, c, col) for nm, t, c, col in zip(names, dtypes, counts, cols)]
+
+
+def _read_ply_fields(path: str):
+    """PLY vertex properties (ascii or binary) -> [(name, numpy type, 1, values (N, 1))]."""
+    with open(path, "rb") as f:
+        if f.readline().strip() != b"ply":
+            raise ValueError(f"{path}: not a PLY file")
+        fmt, n_vertex, props, elements, in_vertex = None, 0, [], [], False
+        while True:
+            line = f.readline()
+            if not line:
+                raise ValueError(f"{path}: truncated PLY header")
+            tok = line.decode("ascii", errors="replace").split()
+            if not tok or tok[0] in ("comment", "obj_info"):
+                continue
+            if tok[0] == "format":
+                fmt = tok[1]
+            elif tok[0] == "element":
+                elements.append(tok[1])
+                in_vertex = tok[1] == "vertex"
+                if in_vertex:
+                    n_vertex = int(tok[2])
+            elif tok[0] == "property" and in_vertex:
+                if tok[1] == "list":
+                    raise ValueError(f"{path}: list properties on vertices are not supported")
+                if tok[1] not in _PLY_TYPES:
+                    raise ValueError(f"{path}: unknown PLY property type {tok[1]}")
+                props.append((tok[2], _PLY_TYPES[tok[1]]))
+            elif tok[0] == "end_header":
+                break
+        if elements and elements[0] != "vertex":
+            raise ValueError(f"{path}: the vertex element must come first")
+        if fmt == "ascii":
+            vals = np.loadtxt(f, dtype=np.float64, max_rows=n_vertex, ndmin=2) if n_vertex else np.zeros((0, len(props)))
+            if vals.shape != (n_vertex, len(props)):
+                raise ValueError(f"{path}: ascii PLY vertex data does not match its header")
+            cols = [vals[:, i : i + 1].astype(t) for i, (_, t) in enumerate(props)]
+        elif fmt in ("binary_little_endian", "binary_big_endian"):
+            order = "<" if fmt == "binary_little_endian" else ">"
+            dt = np.dtype([(f"p{i}", order + t) for i, (_, t) in enumerate(props)])
+            raw = f.read(dt.itemsize * n_vertex)
+            if len(raw) < dt.itemsize * n_vertex:
+                raise ValueError(f"{path}: PLY data holds fewer than the {n_vertex} vertices its header declares")
+            rec = np.frombuffer(raw, dtype=dt, count=n_vertex)
+            cols = [rec[f"p{i}"].astype(t).reshape(n_vertex, 1) for i, (_, t) in enumerate(props)]
+        else:
+            raise ValueError(f"{path}: unknown PLY format {fmt}")
+    return [(nm, t, 1, col) for (nm, t), col in zip(props, cols)]
+
+
+def load_map_cloud(path: str, warn=print) -> np.ndarray:
+    """pcl::io::load(path, PointCloud<PointXYZI>) for a map (preprocess_map.cpp:134), chosen by extension: .pcd (ascii or
+    binary) or .ply (ascii or binary) -> float32 (N, 4) of x, y, z, intensity in file order.
+
+    PCL copies a field into the point only when its name matches, its type is float32 and its count is 1; any other
+    field keeps PointXYZI's default 0 and PCL warns.  Here an x, y or z that does not match (double coordinates, say) is
+    refused, since PCL would silently give zeros; a missing or non-float32 intensity becomes 0 with a warning, as in
+    PCL.  Non-finite coordinates or intensities are refused (the voxel filter and the sort are undefined on them), and
+    so is binary_compressed PCD."""
+    ext = os.path.splitext(path)[1].lower()
+    if ext == ".pcd":
+        fields = _read_pcd_fields(path)
+    elif ext == ".ply":
+        fields = _read_ply_fields(path)
+    else:
+        raise ValueError(f"{path}: unsupported map format {ext or '(no extension)'}; expected .pcd or .ply")
+    n = fields[0][3].shape[0] if fields else 0
+    out = np.zeros((n, 4), dtype=np.float32)
+    for c, name in enumerate(("x", "y", "z", "intensity")):
+        named = [fd for fd in fields if fd[0] == name]
+        match = [fd for fd in named if fd[1] == "f4" and fd[2] in (0, 1)]  # pcl::FieldMatches
+        if match:
+            out[:, c] = match[0][3][:, 0]
+        elif c < 3:
+            got = f"{named[0][1]} x {named[0][2]}" if named else "missing"
+            raise ValueError(f"{path}: field {name} must be float32 with count 1 (got {got}); PCL would silently load zeros for it")
+        else:
+            warn(f"warning: {path}: no float32 intensity field (got {'%s x %d' % named[0][1:3] if named else 'none'}); intensities are 0, as PCL loads them")
+    if not np.all(np.isfinite(out)):
+        bad = int((~np.isfinite(out).all(axis=1)).sum())
+        raise ValueError(f"{path}: {bad} points have a non-finite coordinate or intensity")
+    return out
+
+
 def load_image_gray(path: str) -> np.ndarray:
     """cv::imread(path, 0)."""
     import cv2

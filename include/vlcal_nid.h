@@ -570,6 +570,45 @@ int vlcal_pose_debug_refine(
   int* iterations_out,
   double* final_cost_out);
 
+/* ---- preprocess_map (src/preprocess_map.cpp:34-214, src/vlcal/common/estimate_fov.cpp:53-91) ----------------------------
+ * The GPU stages of building a calibration dataset from a point-cloud map.  Each gives the reference's bits except where
+ * noted; DESIGN §4 "preprocess_map" has the decomposition.  Invalid input (null buffers, negative or too large counts,
+ * non-finite values) gives VLCAL_ERR_INVALID_ARGUMENT with a message.  device = -1: the current device. */
+
+/* pcl::ApproximateVoxelGrid<PointXYZI> with leaf float(leaf_size) (histsize_ 512, downsample_all_data_ true), as
+ * load_lidar_points runs it (preprocess_map.cpp:140-147): sequential over the points in input order, a 512-slot hash of
+ * the voxel index (ix * 7171 + iy * 3079 + iz * 4231) & 511, a slot flushed (centroid / float(count) emitted) when a
+ * point of another voxel arrives, the occupied slots flushed in slot order at the end.  points_xyzi: n x 4 floats
+ * (x, y, z, intensity); points_out: room for n x 4 floats, the centroids in flush order; *n_out their count.
+ * Voxel indices outside int range become INT_MIN as x86-64's float->int conversion gives them (the reference then merges
+ * voxels along that axis); out_of_range_points (optional) counts the points where that happened.  stage_ms_out
+ * (optional, 4 doubles): keys, sort, runs, emission order, between CUDA events.  At most 2^31 - 513 points. */
+int vlcal_approximate_voxel_grid(
+  int device,
+  const float* points_xyzi,
+  int64_t n_points,
+  double leaf_size,
+  float* points_out,
+  int64_t* n_out,
+  int64_t* out_of_range_points,
+  double* stage_ms_out);
+
+/* The rank equalisation of load_lidar_points (preprocess_map.cpp:158-167): with idx sorted by intensity,
+ * intensities_out[idx[i]] = floor(256 * double(i) / n) / 256.  Ties are broken by point index (std::sort leaves them
+ * unspecified; the multiset of outputs is the same).  kernel_ms_out (optional): the GPU time between CUDA events. */
+int vlcal_equalize_intensities(int device, const float* intensities, int64_t n_points, double* intensities_out, double* kernel_ms_out);
+
+/* estimate_lidar_fov's point set before the hull (estimate_fov.cpp:53-66): pcl::VoxelGrid<PointXYZ> at 0.2 m (voxels in
+ * ascending grid index, each the float mean of its points summed in point-index order), or the input itself where the
+ * grid's dx * dy * dz exceeds INT32_MAX (*unfiltered_out = 1, PCL's fallback); then the points with float norm < 1.0
+ * removed, order kept.  points_xyz: n x 3 floats; candidates_out: room for n x 3 floats.  kernel_ms_out optional. */
+int vlcal_lidar_fov_candidates(
+  int device, const float* points_xyz, int64_t n_points, float* candidates_out, int64_t* n_out, int* unfiltered_out, double* kernel_ms_out);
+
+/* min over vertex pairs i < j of dot(dirs_i, dirs_j), dirs = double(vertex).normalized(), starting from M_PI
+ * (estimate_fov.cpp:78-89); never-contracted double, Eigen's left-to-right term order.  Fewer than 2 vertices: M_PI. */
+int vlcal_min_bearing_cosine(int device, const float* vertices_xyz, int64_t n_vertices, double* min_cosine_out);
+
 #ifdef __cplusplus
 }
 #endif
