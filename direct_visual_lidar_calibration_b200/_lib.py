@@ -171,6 +171,9 @@ def load_library():
     L.vlcal_nid_p2p_destroy.restype = None
     L.vlcal_nid_p2p_set_default.argtypes = [vp]
     L.vlcal_nid_set_solver_mode.argtypes = [C.c_int]
+    L.vlcal_nid_debug_record_solve_trace.argtypes = [C.c_int]
+    L.vlcal_nid_debug_last_solve_trace.argtypes = [C.c_int, dp, ip]
+    L.vlcal_nid_debug_last_points_per_lane.argtypes = [vp, ip]
     L.vlcal_view_cull.argtypes = [C.c_int, C.c_int, dp, C.c_int, dp, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, vp, C.c_int64, dp, vp, C.POINTER(C.c_int64)]
     L.vlcal_generate_lidar_image.argtypes = [C.c_int, C.c_int, dp, C.c_int, dp, C.c_int, C.c_int, C.c_int, dp, vp, vp, C.c_int64, vp, vp]
     L.vlcal_nm_default_params.argtypes = [C.POINTER(NMParams)]

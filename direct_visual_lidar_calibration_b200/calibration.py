@@ -201,6 +201,23 @@ class VisualCameraCalibration:
         return colmajor_to_T(out)[0], r
 
 
+def record_solve_trace(enable: bool):
+    """Test hook: keep (True) or stop keeping (False) the evaluations of the calling thread's inner solves for
+    last_solve_trace(); off by default."""
+    _lib.check(_lib.load_library().vlcal_nid_debug_record_solve_trace(int(enable)))
+
+
+def last_solve_trace() -> np.ndarray:
+    """(n, 7) rows {x[6], y}: every evaluation of the calling thread's last Nelder-Mead inner solve, in the reference's
+    order, as its best-cost callback logic saw them (test hook; needs record_solve_trace(True) before the solve)."""
+    L = _lib.load_library()
+    n = C.c_int()
+    _lib.check(L.vlcal_nid_debug_last_solve_trace(0, None, C.byref(n)))
+    rows = np.zeros((n.value, 7))
+    _lib.check(L.vlcal_nid_debug_last_solve_trace(n.value, _dp(rows), C.byref(n)))
+    return rows
+
+
 def estimate_pose_on_costs(costs, init_T_camera_lidar, params: VisualCameraCalibrationParams | None = None, allreduce=None, callback=None):
     """Nelder-Mead over already-built CostCalculatorNID objects (the `costs` vector of visual_camera_calibration.cpp:75-127)."""
     L = _lib.load_library()

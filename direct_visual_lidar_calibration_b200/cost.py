@@ -164,6 +164,12 @@ class CostCalculatorNID:
         _lib.check(self._L.vlcal_nid_debug_solve_stamps(self._ctx, int(capacity), buf, C.byref(n)))
         return np.ctypeslib.as_array(buf).reshape(capacity, 8)[: n.value].copy()
 
+    def last_points_per_lane(self) -> int:
+        """Points per lane (2 or 4) of the kernel instance the last persistent launch on this cost object ran (0: none yet)."""
+        k = C.c_int()
+        _lib.check(self._L.vlcal_nid_debug_last_points_per_lane(self._ctx, C.byref(k)))
+        return int(k.value)
+
     def tma_stats(self):
         """(gathers served by the TMA-staged shared-memory window, gathers that escaped to global memory) of the last persistent solve (VLCAL_PK_TMA=1)."""
         buf = (C.c_uint64 * 2)()

@@ -23,6 +23,8 @@ double now_ms() {
 
 vlcal_p2p* g_default_p2p = nullptr;  // vlcal_nid_p2p_set_default
 int g_solver_mode = 0;                // vlcal_nid_set_solver_mode: 0 auto, 1 host loop, 2 device-resident loop
+thread_local bool g_record_solve_trace = false;  // vlcal_nid_debug_record_solve_trace
+thread_local std::vector<double> g_solve_trace;  // [k][7]: solve_trace_push
 
 // the kernel sums over ranks only when a CONNECTED exchange spanning more than one rank is attached (fill_common_args)
 inline bool ctx_exchange_is_fused(const vlcal_nid_ctx* c) {
@@ -76,6 +78,7 @@ struct PoseObjective {
 
   // the objective's side effects, in the reference's evaluation order (:112-116)
   void observe(const double* x, double y) {
+    solve_trace_push(x, y);
     if (y < best_cost) {
       best_cost = y;
       if (callback) {
@@ -158,6 +161,7 @@ int run_inner_solve_device(
       for (int k = trace_seen; k < count; k++) {
         const double* e = trace + stride * k;
         const double y = e[NM_MAX_N];
+        solve_trace_push(e, y);
         if (y < best_cost) {
           best_cost = y;
           if (callback) {
@@ -196,6 +200,7 @@ int run_inner_solve(
   // summed over bags and ranks, and the Nelder-Mead machine stepped inside the kernel.  Needs what pk_supported checks
   // (float4 clouds, lean classifier, bins <= 32, one camera / image size / device) and no host-side all-reduce callback
   // (a connected peer exchange is summed in-kernel instead).
+  solve_trace_clear();
   bool same_px = true;
   for (int i = 1; i < n_ctxs; i++) same_px = same_px && ctxs[i]->p2p == ctxs[0]->p2p;
   const bool px_fused = n_ctxs >= 1 && ctx_exchange_is_fused(ctxs[0]);
@@ -352,7 +357,31 @@ int check_common(const vlcal_calib_params* params, const double* init_T, double*
 
 }  // namespace
 
+void vlcal::solve_trace_clear() {
+  g_solve_trace.clear();
+}
+
+void vlcal::solve_trace_push(const double* x, double y) {
+  if (!g_record_solve_trace) return;
+  g_solve_trace.insert(g_solve_trace.end(), x, x + 6);
+  g_solve_trace.push_back(y);
+}
+
 extern "C" {
+
+int vlcal_nid_debug_record_solve_trace(int enable) {
+  g_record_solve_trace = enable != 0;
+  g_solve_trace.clear();
+  return VLCAL_OK;
+}
+
+int vlcal_nid_debug_last_solve_trace(int capacity, double* rows_out, int* n_out) {
+  if (capacity < 0 || (capacity > 0 && !rows_out) || !n_out) return VLCAL_ERR_INVALID_ARGUMENT;
+  const int have = static_cast<int>(g_solve_trace.size() / 7);
+  if (capacity > 0) std::memcpy(rows_out, g_solve_trace.data(), sizeof(double) * 7 * static_cast<size_t>(std::min(capacity, have)));
+  *n_out = have;
+  return VLCAL_OK;
+}
 
 int vlcal_nid_set_solver_mode(int mode) {
   if (mode < 0 || mode > 3) {

@@ -994,6 +994,12 @@ int vlcal_nid_debug_tma_stats(vlcal_nid_ctx* ctx, uint64_t stats[2]) {
   return VLCAL_OK;
 }
 
+int vlcal_nid_debug_last_points_per_lane(const vlcal_nid_ctx* ctx, int* k_out) {
+  if (!ctx || !k_out) return VLCAL_ERR_INVALID_ARGUMENT;
+  *k_out = ctx->pk_last_kpt;
+  return VLCAL_OK;
+}
+
 int vlcal_nid_debug_block_times(vlcal_nid_ctx* ctx, int capacity_blocks, uint64_t* times_out, int* n_blocks) {
   if (!ctx || capacity_blocks < 0 || !times_out || !n_blocks) return VLCAL_ERR_INVALID_ARGUMENT;
   const int have = static_cast<int>(ctx->pk_block_times.size() / 4);

@@ -134,6 +134,7 @@ struct vlcal_nid_ctx {
   std::vector<unsigned long long> pk_stamps;
   unsigned long long pk_tma_stats[2] = {0, 0};  // TMA variant, last solve: gathers served by the staged window / escaped to global memory
   std::vector<unsigned long long> pk_block_times;  // [grid][4] of one batch (vlcal_nid_debug_block_times)
+  int pk_last_kpt = 0;  // points per lane of the instance the last persistent launch on this context ran (0: none yet)
 
   ~vlcal_nid_ctx();
 };
@@ -158,4 +159,10 @@ int pk_solve(
   vlcal_nm_result* nm_result);
 // sum over the contexts of calculate(T_p) for a pose list of any length, one launch (hist_out: bag 0's joint histograms)
 int pk_score_poses(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_colmajor, int n_poses, double* nid_out, int32_t* hist_out);
+
+// the evaluations (x[6], y) that the last inner solve of the calling thread passed to its best-cost callback logic, in
+// the reference's order (calibration.cu; recorded only while vlcal_nid_debug_record_solve_trace armed it on that thread,
+// read back by vlcal_nid_debug_last_solve_trace)
+void solve_trace_clear();
+void solve_trace_push(const double* x, double y);
 }  // namespace vlcal

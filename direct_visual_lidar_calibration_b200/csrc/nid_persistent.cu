@@ -304,7 +304,8 @@ int pk_solve(
   VL_CUDA(cudaMemsetAsync(scratch.p, 0, L.total, c0->stream));
 
   // host-visible outcome: result + done / error words + evaluation trace, one pinned allocation
-  const int trace_cap = 16 + std::max(0, params->max_inner_iterations) * 8;  // <= 7 evaluations per batch, one batch per iteration (+ shrinks)
+  // n + 1 evaluations of the initial simplex, then at most n + 3 per iteration: xo, xr, xc and the n shrunk vertices
+  const int trace_cap = 7 + std::max(0, params->max_inner_iterations) * 9;
   const size_t trace_bytes = sizeof(double) * (NM_MAX_N + 1) * static_cast<size_t>(trace_cap);
   const size_t head_bytes = (sizeof(PkResult) + sizeof(PkSolve) + 64 + 255) & ~static_cast<size_t>(255);
   PinBuf host;
@@ -421,13 +422,14 @@ int pk_solve(
 
   const NmMachine& fin = h_result->nm;
   // the objective's side effects in the reference's evaluation order (:112-116)
-  if (callback) {
+  {
     double best_cost = DBL_MAX;  // :101
     const int count = std::min(h_result->trace_count, trace_cap);
     for (int k = 0; k < count; k++) {
       const double* e = h_trace + static_cast<size_t>(k) * (NM_MAX_N + 1);
       const double y = e[NM_MAX_N];
-      if (y < best_cost) {
+      solve_trace_push(e, y);
+      if (y < best_cost && callback) {
         best_cost = y;
         double E[16], T[16];
         host::se3_expmap_gtsam(e, E);
@@ -450,6 +452,7 @@ int pk_solve(
     nm_result->num_evaluations_computed = fin.num_evaluations_computed;
   }
   // profile: one launch carried `batches` passes over the cloud(s)
+  for (int i = 0; i < n_ctxs; i++) ctxs[i]->pk_last_kpt = pk_kernel_k(c0->cam.model, kpt);
   c0->launches += 1;
   c0->passes += static_cast<int64_t>(h_result->batches);
   for (int i = 0; i < 4; i++) c0->delta_stats[i] += static_cast<int64_t>(delta_stats[i]);
@@ -561,6 +564,7 @@ int pk_score_poses(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_colma
       nid_out[p] = s;
     }
   }
+  for (int i = 0; i < n_ctxs; i++) ctxs[i]->pk_last_kpt = pk_kernel_k(c0->cam.model, kpt);
   c0->launches += 1;
   c0->passes += n_chunks;
   for (int i = 0; i < 4; i++) c0->delta_stats[i] += static_cast<int64_t>(delta_stats[i]);

@@ -282,6 +282,14 @@ int vlcal_generate_lidar_image(
  * removes), hence the default; with mode 2 params.callback is delivered from the evaluation trace, in
  * the reference's order, up to one chunk of launches late. */
 int vlcal_nid_set_solver_mode(int mode);
+/* test hook: with recording armed on the calling thread (enable != 0; off by default, 0 turns it off again), every inner
+ * solve (vlcal_estimate_pose_nelder_mead*, any solver mode) run on that thread keeps its evaluations as the best-cost
+ * callback logic saw them, in the reference's order; vlcal_nid_debug_last_solve_trace returns those of the last solve --
+ * capacity x 7 doubles {x[6], y} out, *n_out = the solve's count (may exceed capacity) */
+int vlcal_nid_debug_record_solve_trace(int enable);
+int vlcal_nid_debug_last_solve_trace(int capacity, double* rows_out, int* n_out);
+/* test hook: points per lane (2 or 4) of the kernel instance the last persistent launch on this context ran (0: none yet) */
+int vlcal_nid_debug_last_points_per_lane(const vlcal_nid_ctx* ctx, int* k_out);
 
 /* dfo::NelderMead<N>::Params (include/dfo/nelder_mead.hpp:11-22) */
 typedef struct {
