@@ -107,6 +107,14 @@ class PoseEstimationStats(C.Structure):
     ]
 
 
+class ScanDesc(C.Structure):
+    """vlcal_scan_desc: one PointCloud2 scan inside the concatenated data of a bag."""
+    _fields_ = [
+        ("byte_offset", C.c_int64), ("n_points", C.c_int64), ("point_step", C.c_int32), ("x_offset", C.c_int32), ("y_offset", C.c_int32),
+        ("z_offset", C.c_int32), ("xyz_type", C.c_int32), ("intensity_offset", C.c_int32), ("intensity_type", C.c_int32), ("reserved", C.c_int32),
+    ]
+
+
 SE3_OBJECTIVE = C.CFUNCTYPE(C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_void_p)
 NM_BATCH_FN = C.CFUNCTYPE(None, C.POINTER(C.c_double), C.c_int, C.c_int, C.POINTER(C.c_double), C.c_void_p)
 NM_OBSERVE_FN = C.CFUNCTYPE(None, C.POINTER(C.c_double), C.c_int, C.c_double, C.c_void_p)
@@ -202,6 +210,7 @@ def load_library():
     L.vlcal_equalize_intensities.argtypes = [C.c_int, vp, C.c_int64, vp, dp]
     L.vlcal_lidar_fov_candidates.argtypes = [C.c_int, vp, C.c_int64, vp, i64p, ip, dp]
     L.vlcal_min_bearing_cosine.argtypes = [C.c_int, vp, C.c_int64, dp]
+    L.vlcal_bag_integrate.argtypes = [C.c_int, vp, C.c_int64, C.POINTER(ScanDesc), C.c_int64, C.c_double, C.c_double, vp, i64p, i64p, dp]
     _lib = L
     return L
 

@@ -262,3 +262,71 @@ def preprocess_map(map_path: str, image_path: str, dst_path: str, camera_model: 
     stats.update(map_points=int(cloud.shape[0]), filtered=int(filtered.shape[0]), lidar_fov=lidar_fov, virtual_camera=model,
                  voxel_grid=avg_stats, equalize=eq_stats, fov=fov_stats)
     return config
+
+
+# ---- `preprocess` on the command line of the reference (src/vlcal/preprocess/preprocess.cpp:37-82) ----------------------
+
+def build_parser():
+    import argparse
+
+    ap = argparse.ArgumentParser(prog="preprocess", description="calibration dataset from a directory of ROS 1 / ROS 2 (sqlite3) bags")
+    ap.add_argument("data_path", nargs="?", help="directory that contains rosbags for calibration")
+    ap.add_argument("dst_path", nargs="?", help="directory to save preprocessed data")
+    ap.add_argument("--bag_id", type=int, help="specify the bag to use (just for evaluation)")
+    ap.add_argument("--first_n_bags", type=int, help="use only the first N bags (just for evaluation)")
+    ap.add_argument("-a", "--auto_topic", action="store_true", help="automatically select topics")
+    ap.add_argument("-d", "--dynamic_lidar_integration", action="store_true", help="not supported: only the static integrator is implemented")
+    ap.add_argument("-i", "--intensity_channel", default="auto", help="auto or channel name")
+    ap.add_argument("--camera_info_topic")
+    ap.add_argument("--image_topic")
+    ap.add_argument("--points_topic")
+    ap.add_argument("--camera_model", default="auto", help="auto, plumb_bob, fisheye(=equidistant), omnidir, or equirectangular")
+    ap.add_argument("--camera_intrinsics", help="camera intrinsic parameters [fx,fy,cx,cy(,xi)] (don't put spaces between values!!)")
+    ap.add_argument("--camera_distortion_coeffs", help="camera distortion parameters [k1,k2,p1,p2,k3] (don't put spaces between values!!)")
+    ap.add_argument("--k_neighbors", type=int, default=20, help="used by the dynamic integrator only")
+    ap.add_argument("--voxel_resolution", type=float, default=0.002, help="voxel grid resolution")
+    ap.add_argument("--min_distance", type=float, default=1.0, help="minimum point distance. Points closer than this value will be discarded")
+    ap.add_argument("--verbose", action="store_true")
+    ap.add_argument("-v", "--visualize", action="store_true", help="no viewer here: prints a note and continues")
+    ap.add_argument("--device", type=int, default=-1, help="CUDA device (-1: the current one)")
+    return ap
+
+
+def main(argv=None) -> int:
+    """python -m direct_visual_lidar_calibration_b200.preprocess <data_path> <dst_path> [flags].  As in the reference, a
+    missing path prints the usage and exits 0."""
+    import sys
+
+    from . import bag_io
+    from . import preprocess_bag as PB
+
+    ap = build_parser()
+    args = ap.parse_args(argv)
+    if args.data_path is None or args.dst_path is None:
+        ap.print_help()
+        return 0
+    if args.dynamic_lidar_integration:
+        bags = PB.list_bags(args.data_path) if os.path.isdir(args.data_path) else []
+        names = ", ".join(os.path.basename(b) for b in bags) or args.data_path
+        print(f"error: {names}: dynamic LiDAR integration (-d, CT-GICP odometry) is not supported; only the static integrator is",
+              file=sys.stderr)
+        return 1
+    if args.visualize:
+        print("note: there is no viewer (-v); continuing without it")
+    print(f"data_path: {args.data_path}\ndst_path : {args.dst_path}")
+    try:
+        PB.preprocess_bags(args.data_path, args.dst_path, auto_topic=args.auto_topic, camera_info_topic=args.camera_info_topic,
+                           image_topic=args.image_topic, points_topic=args.points_topic, intensity_channel=args.intensity_channel,
+                           camera_model=args.camera_model, camera_intrinsics=args.camera_intrinsics,
+                           camera_distortion_coeffs=args.camera_distortion_coeffs, voxel_resolution=args.voxel_resolution,
+                           min_distance=args.min_distance, bag_id=args.bag_id, first_n_bags=args.first_n_bags, device=args.device)
+    except (ValueError, FileNotFoundError, bag_io.BagError) as e:
+        print(f"error: {e}", file=sys.stderr)
+        return 1
+    return 0
+
+
+if __name__ == "__main__":
+    import sys
+
+    sys.exit(main())

@@ -617,6 +617,44 @@ int vlcal_lidar_fov_candidates(
  * (estimate_fov.cpp:78-89); never-contracted double, Eigen's left-to-right term order.  Fewer than 2 vertices: M_PI. */
 int vlcal_min_bearing_cosine(int device, const float* vertices_xyz, int64_t n_vertices, double* min_cosine_out);
 
+/* ---- preprocess from bags (src/vlcal/preprocess/preprocess.cpp:406-476) -------------------------------------------------
+ * One accepted sensor_msgs/PointCloud2 scan of a bag: its little-endian `data` starts at byte_offset of the concatenated
+ * blob and holds n_points = width * height points of point_step bytes.  Datatypes are PointField's: xyz_type 7 (FLOAT32)
+ * or 8 (FLOAT64) -- x's datatype, with which y and z are read as the reference reads them; intensity_type 2, 4, 6, 7
+ * or 8 (UINT8, UINT16, UINT32, FLOAT32, FLOAT64).  Offsets need not be aligned. */
+typedef struct {
+  int64_t byte_offset;
+  int64_t n_points;
+  int32_t point_step;
+  int32_t x_offset;
+  int32_t y_offset;
+  int32_t z_offset;
+  int32_t xyz_type;
+  int32_t intensity_offset;
+  int32_t intensity_type;
+  int32_t reserved;
+} vlcal_scan_desc;
+
+/* extract_raw_points, the finiteness filter and StaticPointCloudIntegrator::insert_points / get_points over every point
+ * of the scans in order (DESIGN §4c): points with a non-finite coordinate or a norm below min_distance are dropped, the
+ * rest written to the voxel floor(p / voxel_resolution) (double, cast to int; out of int range gives INT_MIN as on
+ * x86-64, counted in out_of_range_points), the last point written to a voxel wins.  points_out: room for 4 floats per
+ * input point; receives (float(x), float(y), float(z), float(intensity)) of the winners in first-write order (the order
+ * in which their voxels were first written; the reference's is its hash table's), *n_out of them.  stage_ms_out
+ * (optional, 3 doubles): decode, sort, runs + emission, between CUDA events.  At most 2^31 - 1 points. */
+int vlcal_bag_integrate(
+  int device,
+  const uint8_t* data,
+  int64_t data_bytes,
+  const vlcal_scan_desc* scans,
+  int64_t n_scans,
+  double voxel_resolution,
+  double min_distance,
+  float* points_out,
+  int64_t* n_out,
+  int64_t* out_of_range_points,
+  double* stage_ms_out);
+
 #ifdef __cplusplus
 }
 #endif
