@@ -183,6 +183,8 @@ def load_library():
     L.vlcal_nid_debug_last_solve_trace.argtypes = [C.c_int, dp, ip]
     L.vlcal_nid_debug_last_points_per_lane.argtypes = [vp, ip]
     L.vlcal_view_cull.argtypes = [C.c_int, C.c_int, dp, C.c_int, dp, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, vp, C.c_int64, dp, vp, C.POINTER(C.c_int64)]
+    L.vlcal_debug_view_cull_points.argtypes = [C.c_int, C.c_int, dp, C.c_int, dp, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_int, vp, vp, C.c_int64, dp, vp,
+                                               C.POINTER(C.c_int64), ip]
     L.vlcal_generate_lidar_image.argtypes = [C.c_int, C.c_int, dp, C.c_int, dp, C.c_int, C.c_int, C.c_int, dp, vp, vp, C.c_int64, vp, vp]
     L.vlcal_nm_default_params.argtypes = [C.POINTER(NMParams)]
     L.vlcal_nm_default_params.restype = None

@@ -363,3 +363,57 @@ extern "C" int vlcal_view_cull(
   if (rc != VLCAL_OK) return rc;
   return view_cull_device(cam, width, height, max_fov_rad, enable_depth_buffer_culling != 0, *cloud, T_camera_lidar, nullptr, nullptr, indices_out, n_kept, false);
 }
+
+extern "C" int vlcal_debug_view_cull_points(
+  int device,
+  int camera_model,
+  const double* intrinsics,
+  int n_intrinsics,
+  const double* distortion,
+  int n_distortion,
+  int width,
+  int height,
+  double max_fov_rad,
+  int enable_depth_buffer_culling,
+  int keep_all,
+  const double* points_xyzw,
+  const double* intensities,
+  int64_t n_points,
+  const double T_camera_lidar[16],
+  double* points_out,
+  int64_t* n_kept,
+  int* points_are_f32) {
+  if (width <= 0 || height <= 0 || n_points < 0 || (n_points > 0 && (!points_xyzw || !intensities || !points_out)) || !T_camera_lidar || !n_kept) {
+    set_last_error("invalid arguments");
+    return VLCAL_ERR_INVALID_ARGUMENT;
+  }
+  CameraParams cam;
+  int rc = make_camera(camera_model, intrinsics, n_intrinsics, distortion, n_distortion, &cam);
+  if (rc != VLCAL_OK) return rc;
+  if (vlcal_nid_device_count() == 0) {
+    set_last_error("no CUDA device available: this library has no CPU fallback");
+    return VLCAL_ERR_NO_DEVICE;
+  }
+  if (device < 0) VL_CUDA(cudaGetDevice(&device));
+  VL_CUDA(cudaSetDevice(device));
+  if (max_fov_rad < 0.0) max_fov_rad = estimate_camera_fov_host(cam, width, height);
+  std::shared_ptr<DeviceCloud> cloud, culled;
+  rc = upload_cloud(device, points_xyzw, intensities, n_points, nullptr, &cloud);
+  if (rc != VLCAL_OK) return rc;
+  if (points_are_f32) *points_are_f32 = cloud->f32 ? 1 : 0;
+  // culled_out without an index list: the paths of the cost objects (tile-ordered counting sort, or the keep_all reorder)
+  rc = view_cull_device(cam, width, height, max_fov_rad, enable_depth_buffer_culling != 0, *cloud, T_camera_lidar, nullptr, &culled, nullptr, n_kept, keep_all != 0);
+  if (rc != VLCAL_OK) return rc;
+  const size_t kept = static_cast<size_t>(culled->n);
+  if (kept == 0) return VLCAL_OK;
+  if (culled->f32) {
+    std::vector<float4> h(kept);
+    VL_CUDA(cudaMemcpy(h.data(), culled->d_points, sizeof(float4) * kept, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < kept; i++) {
+      points_out[4 * i] = h[i].x, points_out[4 * i + 1] = h[i].y, points_out[4 * i + 2] = h[i].z, points_out[4 * i + 3] = h[i].w;
+    }
+  } else {
+    VL_CUDA(cudaMemcpy(points_out, culled->d_points, sizeof(double4) * kept, cudaMemcpyDeviceToHost));
+  }
+  return VLCAL_OK;
+}

@@ -244,6 +244,30 @@ int vlcal_view_cull(
   const double T_camera_lidar[16],
   int32_t* indices_out,
   int64_t* n_kept);
+/* test hook: view culling as the cost objects of the solver run it, with the culled cloud kept on the device and no index
+ * list.  keep_all == 0: the kept points grouped by 32 x 8-pixel image tile at T (the cloud vlcal_calibrate_nelder_mead
+ * scores); keep_all != 0: every point, grouped the same way, the ones out of view last (vlcal_nid_reorder_for_pose).
+ * points_out: capacity n_points x 4 doubles, receives (x, y, z, intensity) of the culled cloud in its device order;
+ * *n_kept its count; *points_are_f32 (may be NULL): 1 if the cloud went to the device in the float4 layout. */
+int vlcal_debug_view_cull_points(
+  int device,
+  int camera_model,
+  const double* intrinsics,
+  int n_intrinsics,
+  const double* distortion,
+  int n_distortion,
+  int width,
+  int height,
+  double max_fov_rad,
+  int enable_depth_buffer_culling,
+  int keep_all,
+  const double* points_xyzw,
+  const double* intensities,
+  int64_t n_points,
+  const double T_camera_lidar[16],
+  double* points_out,
+  int64_t* n_kept,
+  int* points_are_f32);
 
 /* ---- LiDAR intensity image: vlcal::generate_lidar_image (src/vlcal/preprocess/generate_lidar_image.cpp:8-41) ----------
  * The rendering `preprocess` / `initial_guess_*` use: per pixel the projected point with the smallest squared range (of

@@ -70,7 +70,7 @@ def test_histograms_bit_exact_vs_oracle(gpu, oracle, model):
 
 def test_batch_equals_singles_and_chunking(gpu, oracle):
     pr = util.random_problem("plumb_bob", n=30000, seed=5)
-    Ts = util.random_poses(pr["T"], 21, seed=8)  # > 2 launches of 8 poses
+    Ts = util.random_poses(pr["T"], 21, seed=8)  # three passes of the persistent kernel (the round-1 chunking: test_gpu_round1_edges.py)
     cost = _cost(gpu, pr)
     nid, hist = cost.calculate_batch(Ts, return_hist=True)
     for p in (0, 7, 8, 20):
