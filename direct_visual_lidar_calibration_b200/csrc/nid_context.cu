@@ -602,6 +602,7 @@ int nid_evaluate_async(vlcal_nid_ctx* ctx, const double* T_colmajor, int n_poses
   }
   ctx->seq += 1;
   ctx->in_flight = true;
+  ctx->in_flight_hist = want_hist;
   ctx->in_flight_poses = n_poses;
   return VLCAL_OK;
 }
@@ -718,7 +719,9 @@ int nid_wait(vlcal_nid_ctx* ctx, double* nid_out, int32_t* hist_out) {
   const int n_poses = ctx->in_flight_poses;
   if (nid_out) std::memcpy(nid_out, ctx->h_nid, sizeof(double) * n_poses);
   if (hist_out) {
-    if (!ctx->d_hist_out) {
+    // d_hist_out outlives the evaluation that filled it: without this check an evaluation that did not request
+    // histograms would hand back the previous one's
+    if (!ctx->in_flight_hist) {
       set_last_error("histograms were not requested for the evaluation in flight");
       return VLCAL_ERR_INVALID_ARGUMENT;
     }

@@ -111,6 +111,7 @@ struct vlcal_nid_ctx {
   int num_sms = 132;  // read from the device at create
   // async state
   bool in_flight = false;
+  bool in_flight_hist = false;  // the evaluation in flight writes its histograms to d_hist_out
   int in_flight_poses = 0;
   vlcal_p2p* p2p = nullptr;  // attached peer exchange (not owned)
   // debug timeline (vlcal_nid_debug_timeline)

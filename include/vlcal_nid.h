@@ -116,7 +116,8 @@ int vlcal_nid_evaluate(vlcal_nid_ctx* ctx, const double* T_camera_lidar, int n_p
 
 /* same, split so that several contexts (bags) overlap on the GPU: _async enqueues on the context's stream and
  * returns; _wait blocks until that evaluation is done and delivers the results. One evaluation in flight per
- * context (VLCAL_ERR_BUSY otherwise). */
+ * context (VLCAL_ERR_BUSY otherwise).  _async computes no histograms: after it, _wait's hist_out must be NULL
+ * (VLCAL_ERR_INVALID_ARGUMENT otherwise; the scores are still delivered and the evaluation is no longer in flight). */
 int vlcal_nid_evaluate_async(vlcal_nid_ctx* ctx, const double* T_camera_lidar, int n_poses);
 int vlcal_nid_wait(vlcal_nid_ctx* ctx, double* nid_out, int32_t* hist_out);
 
