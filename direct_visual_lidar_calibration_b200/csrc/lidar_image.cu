@@ -129,6 +129,11 @@ extern "C" int vlcal_generate_lidar_image(
     set_last_error("invalid arguments (at most 2^31-1 points: the index map is CV_32SC1)");
     return VLCAL_ERR_INVALID_ARGUMENT;
   }
+  // pixel indices are int (exact_pixel_hd returns iy * width + ix): refused before anything is uploaded or allocated
+  if (static_cast<int64_t>(width) * height > 0x7fffffffLL) {
+    set_last_error("invalid arguments (at most 2^31-1 pixels: width * height = " + std::to_string(static_cast<int64_t>(width) * height) + ")");
+    return VLCAL_ERR_INVALID_ARGUMENT;
+  }
   CameraParams cam;
   int rc = make_camera(camera_model, intrinsics, n_intrinsics, distortion, n_distortion, &cam);
   if (rc != VLCAL_OK) return rc;

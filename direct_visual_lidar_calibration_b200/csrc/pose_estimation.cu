@@ -83,7 +83,7 @@ struct PoseScoreArgs {
 };
 
 __device__ __forceinline__ bool load_rotation(const PoseScoreArgs& a, int2 ij, xd R[9]) {
-  const int m = a.m;
+  const long long m = a.m;  // 2m + i exceeds INT_MAX above 2^30 correspondences
   const double c1[3] = {a.dc[ij.x], a.dc[m + ij.x], a.dc[2 * m + ij.x]};
   const double c2[3] = {a.dc[ij.y], a.dc[m + ij.y], a.dc[2 * m + ij.y]};
   const double l1[3] = {a.dl[ij.x], a.dl[m + ij.x], a.dl[2 * m + ij.x]};
@@ -569,9 +569,9 @@ int vlcal_estimate_pose_from_correspondences(
   if (rc != VLCAL_OK) return rc;
 
   // [R_ransac | 0] (:24-25), R recomputed on the host: the same operations give the same bits as on the device
-  const int i1 = pairs[2 * best], i2 = pairs[2 * best + 1];
-  const double c1[3] = {b.dc[i1], b.dc[m + i1], b.dc[2 * static_cast<size_t>(m) + i1]}, c2[3] = {b.dc[i2], b.dc[m + i2], b.dc[2 * static_cast<size_t>(m) + i2]};
-  const double l1[3] = {b.dl[i1], b.dl[m + i1], b.dl[2 * static_cast<size_t>(m) + i1]}, l2[3] = {b.dl[i2], b.dl[m + i2], b.dl[2 * static_cast<size_t>(m) + i2]};
+  const size_t i1 = static_cast<size_t>(pairs[2 * best]), i2 = static_cast<size_t>(pairs[2 * best + 1]), mm = static_cast<size_t>(m);
+  const double c1[3] = {b.dc[i1], b.dc[mm + i1], b.dc[2 * mm + i1]}, c2[3] = {b.dc[i2], b.dc[mm + i2], b.dc[2 * mm + i2]};
+  const double l1[3] = {b.dl[i1], b.dl[mm + i1], b.dl[2 * mm + i1]}, l2[3] = {b.dl[i2], b.dl[mm + i2], b.dl[2 * mm + i2]};
   xd R[9];
   pair_rotation(c1, c2, l1, l2, R);
   double T0[16];

@@ -274,7 +274,8 @@ int vlcal_debug_view_cull_points(
  * The rendering `preprocess` / `initial_guess_*` use: per pixel the projected point with the smallest squared range (of
  * equal ones the last), same FoV / projection / truncation rules as the NID cost, FoV from estimate_camera_fov(camera,
  * {width, height}).  intensity_image_out: H x W doubles (CV_64FC1; 0 where no point lands), index_image_out: H x W int32
- * (CV_32SC1; -1 where no point lands).  Exact: both images equal the reference's bit for bit. */
+ * (CV_32SC1; -1 where no point lands).  Exact: both images equal the reference's bit for bit.  At most 2^31-1 points and
+ * 2^31-1 pixels (width * height); larger inputs are refused with VLCAL_ERR_INVALID_ARGUMENT before anything is allocated. */
 int vlcal_generate_lidar_image(
   int device,
   int camera_model,

@@ -3,8 +3,8 @@
  *
  * A plain-C restatement, linked against the CPU oracle (oracle/vlcal_oracle.c: orc_project, orc_nelder_mead), of
  *   - estimate_direction (src/vlcal/common/estimate_fov.cpp:17-34) and the LiDAR bearings (estimate_pose.cpp:47-51);
- *   - the per-hypothesis rotation (the closed-form two-pair Umeyama solution) and inlier count (:108-116), in the
- *     operation order of the kernel, so that every squared error equals the kernel's up to the last-ulp differences of
+ *   - the per-hypothesis rotation (the closed-form two-pair Umeyama solution), the squared reprojection errors and the
+ *     inlier count (:108-116), in the operation order of the kernel, so that every squared error equals the kernel's up to the last-ulp differences of
  *     the device's transcendental functions (fisheye, atan, equirectangular);
  *   - InitialGuessAuto::read_correspondences' rules (initial_guess_auto.cpp:81-125).
  * Built with -ffp-contract=off (no FMA), like the oracle.
@@ -87,6 +87,25 @@ void pose_oracle_bearings(const orc_camera* cam, const double* kp0, const double
   }
 }
 
+/* the kernel's rotation of one hypothesis from its two bearing pairs (c_k = R l_k): 1 and R (row-major), or 0 where the
+ * pair is degenerate (R untouched) */
+int pose_oracle_rotation(const double c1[3], const double c2[3], const double l1[3], const double l2[3], double R[9]) { return pair_rotation(c1, c2, l1, l2, R); }
+
+/* |kp0_j - project(R dl_j)|^2 (:110-113), in the kernel's operation order */
+static double sq_error(const orc_camera* cam, const double R[9], const double* kp, const double* d) {
+  const double pc[3] = {(R[0] * d[0] + R[1] * d[1]) + R[2] * d[2], (R[3] * d[0] + R[4] * d[1]) + R[5] * d[2], (R[6] * d[0] + R[7] * d[1]) + R[8] * d[2]};
+  double uv[2];
+  orc_project(cam, pc, uv);
+  const double du = kp[0] - uv[0], dv = kp[1] - uv[1];
+  return du * du + dv * dv;
+}
+
+/* e[j] = the squared reprojection error of every correspondence under R: correspondence j is an inlier iff e[j] < thresh^2 */
+void pose_oracle_errors(const orc_camera* cam, const double R[9], const double* kp0, const double* dl, int m, double* e) {
+#pragma omp parallel for schedule(static)
+  for (int j = 0; j < m; j++) e[j] = sq_error(cam, R, kp0 + 2 * j, dl + 3 * j);
+}
+
 /* per hypothesis h: counts[h] = #{j : |kp0_j - project(R_h dl_j)|^2 < thresh^2}, degenerate[h], near[h] = #{j : the squared
  * error lies within 1e-9 px^2 of thresh^2} (where device and host transcendental functions may decide differently) */
 void pose_oracle_score(
@@ -101,12 +120,7 @@ void pose_oracle_score(
     degenerate[k] = ok ? 0 : 1;
     int count = 0, close = 0;
     for (int j = 0; ok && j < m; j++) {
-      const double* d = dl + 3 * j;
-      const double pc[3] = {(R[0] * d[0] + R[1] * d[1]) + R[2] * d[2], (R[3] * d[0] + R[4] * d[1]) + R[5] * d[2], (R[6] * d[0] + R[7] * d[1]) + R[8] * d[2]};
-      double uv[2];
-      orc_project(cam, pc, uv);
-      const double du = kp0[2 * j] - uv[0], dv = kp0[2 * j + 1] - uv[1];
-      const double e = du * du + dv * dv;
+      const double e = sq_error(cam, R, kp0 + 2 * j, dl + 3 * j);
       count += e < thresh_sq;
       close += fabs(e - thresh_sq) <= 1e-9;
     }

@@ -31,6 +31,9 @@ def lib():
         L.pose_oracle_direction.argtypes = [cam, dp, dp]
         L.pose_oracle_bearings.argtypes = [cam, dp, dp, C.c_int, dp, dp]
         L.pose_oracle_score.argtypes = [cam, dp, dp, dp, C.c_int, vp, C.c_int, C.c_double, vp, vp, vp]
+        L.pose_oracle_rotation.argtypes = [dp, dp, dp, dp, dp]
+        L.pose_oracle_rotation.restype = C.c_int
+        L.pose_oracle_errors.argtypes = [cam, dp, dp, dp, C.c_int, dp]
         L.pose_oracle_correspondences.argtypes = [vp, C.c_int, C.c_int, dp, C.c_int, dp, C.c_int, dp, C.c_int64, vp, vp, C.POINTER(C.c_int)]
         _lib = L
     return _lib
@@ -53,11 +56,43 @@ def score(cam, kp0, points, pairs, thresh):
     """-> (counts, degenerate, near-threshold counts) per hypothesis"""
     kp = np.ascontiguousarray(kp0, dtype=np.float64)
     dc, dl = bearings(cam, kp, points)
+    return score_bearings(cam, kp, dc, dl, pairs, thresh)
+
+
+def score_bearings(cam, kp0, dc, dl, pairs, thresh):
+    """score() on bearings computed once with bearings()"""
+    kp = np.ascontiguousarray(kp0, dtype=np.float64)
+    dc, dl = np.ascontiguousarray(dc, dtype=np.float64), np.ascontiguousarray(dl, dtype=np.float64)
     pr = np.ascontiguousarray(pairs, dtype=np.int32)
     h = pr.shape[0]
     counts, degenerate, near = np.empty(h, np.int32), np.empty(h, np.uint8), np.empty(h, np.int32)
     lib().pose_oracle_score(C.byref(cam), _dp(kp), _dp(dc), _dp(dl), kp.shape[0], pr.ctypes.data, h, float(thresh), counts.ctypes.data, degenerate.ctypes.data, near.ctypes.data)
     return counts, degenerate.astype(bool), near
+
+
+def rotation(c1, c2, l1, l2):
+    """The kernel's rotation R (3x3, c_k = R l_k) of one hypothesis from its two bearing pairs, or None where the pair is
+    degenerate."""
+    v = [np.ascontiguousarray(np.asarray(x, dtype=np.float64).reshape(3)) for x in (c1, c2, l1, l2)]
+    R = np.empty(9)
+    ok = lib().pose_oracle_rotation(*[_dp(x) for x in v], _dp(R))
+    return R.reshape(3, 3) if ok else None
+
+
+def pair_rotation(dc, dl, pair):
+    """rotation() of the index pair (i, j) of bearings (M,3); None where the RANSAC rule calls it degenerate (i == j too)."""
+    i, j = int(pair[0]), int(pair[1])
+    return None if i == j else rotation(dc[i], dc[j], dl[i], dl[j])
+
+
+def errors(cam, R, kp0, dl):
+    """-> e (M,): |kp0_j - project(R dl_j)|^2 in the kernel's order; correspondence j is an inlier iff e[j] < pow(thresh, 2)."""
+    kp = np.ascontiguousarray(kp0, dtype=np.float64)
+    d = np.ascontiguousarray(dl, dtype=np.float64)
+    Rf = np.ascontiguousarray(np.asarray(R, dtype=np.float64).reshape(9))
+    e = np.empty(kp.shape[0])
+    lib().pose_oracle_errors(C.byref(cam), _dp(Rf), _dp(kp), _dp(d), kp.shape[0], _dp(e))
+    return e
 
 
 def correspondences(index_image, kpts0, kpts1, matches, n_points):
