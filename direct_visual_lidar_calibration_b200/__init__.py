@@ -12,6 +12,7 @@ this package is the thin host-side mirror of the reference's interface for that 
   VisualCameraCalibrationParams, VisualCameraCalibration <- vlcal::VisualCameraCalibration
                                                                      (include/vlcal/calib/visual_camera_calibration.hpp)
   PoseEstimationParams, PoseEstimation <- vlcal::PoseEstimation      (include/vlcal/common/estimate_pose.hpp)
+  PointsColorUpdater            <- vlcal::PointsColorUpdater         (include/vlcal/common/points_color_updater.hpp)
 
 There is no CPU fallback: without the built library or without a CUDA device every compute call raises.
 """
@@ -23,6 +24,7 @@ from .nelder_mead import NelderMead, NelderMeadParams
 from . import bfgs
 from .calibration import RegistrationType, VisualCameraCalibration, VisualCameraCalibrationParams, estimate_camera_fov, se3_expmap
 from .pose_estimation import PoseEstimation, PoseEstimationParams
+from .points_color_updater import PointsColorUpdater, render_overlay, turbo_colormap
 
 __all__ = [
     "score_poses",
@@ -34,4 +36,5 @@ __all__ = [
     "NelderMead", "NelderMeadParams",
     "RegistrationType", "VisualCameraCalibration", "VisualCameraCalibrationParams", "estimate_camera_fov", "se3_expmap",
     "PoseEstimation", "PoseEstimationParams",
+    "PointsColorUpdater", "render_overlay", "turbo_colormap",
 ]

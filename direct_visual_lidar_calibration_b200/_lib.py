@@ -186,6 +186,10 @@ def load_library():
     L.vlcal_debug_view_cull_points.argtypes = [C.c_int, C.c_int, dp, C.c_int, dp, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_int, vp, vp, C.c_int64, dp, vp,
                                                C.POINTER(C.c_int64), ip]
     L.vlcal_generate_lidar_image.argtypes = [C.c_int, C.c_int, dp, C.c_int, dp, C.c_int, C.c_int, C.c_int, dp, vp, vp, C.c_int64, vp, vp]
+    viewer = [C.c_int, C.c_int, dp, C.c_int, dp, C.c_int, C.c_int, C.c_int, vp, C.c_int, dp, vp, vp, C.c_int64]
+    L.vlcal_turbo_colormap.argtypes = [vp]
+    L.vlcal_colorize_points.argtypes = viewer + [C.c_float, vp, dp]
+    L.vlcal_render_overlay.argtypes = viewer + [C.c_int, C.c_float, vp, vp, dp]
     L.vlcal_nm_default_params.argtypes = [C.POINTER(NMParams)]
     L.vlcal_nm_default_params.restype = None
     L.vlcal_nelder_mead_batched.argtypes = [C.c_int, NM_BATCH_FN, NM_OBSERVE_FN, vp, dp, C.POINTER(NMParams), C.POINTER(NMResult)]

@@ -9,6 +9,9 @@
 //      non-negative double per pixel;
 //   2. points whose squared range equals their pixel's minimum: atomicMax of the point index;
 //   3. per pixel: intensity of the winning point (0 / -1 where nothing landed, :13-15).
+// Passes 1 and 2 take a radius: a point then competes for the (2r+1)^2 square of pixels around its own, clipped to the
+// image.  The reference's image is radius 0; the viewer's overlay (viewer.cu) draws with a larger one through the same
+// routine, lidar_index_image_passes.
 #include <cstring>
 
 #include "exact_classify.cuh"
@@ -21,6 +24,7 @@ struct LidarImageArgs {
   const void* points;  // float4 (x, y, z, intensity) or double4
   long long n;
   int width, height;
+  int radius;  // a point covers pixels within `radius` of its own in x and y (0: the reference's rendering)
   double cos_fov;
   CameraParams cam;
   double pose[12];
@@ -28,8 +32,21 @@ struct LidarImageArgs {
   int* pix;                  // [n] pixel of every point, -1 if the reference skips it
   double* sq_dist;           // [n]
   int* index_image;          // [H*W], initialised to -1 (:15)
-  double* intensity_image;   // [H*W]
 };
+
+// f(pixel) for every pixel of the square of `radius` around pixel `pix`, clipped to the image
+template <class F>
+__device__ __forceinline__ void for_each_covered_pixel(int pix, int radius, int width, int height, F f) {
+  if (radius == 0) {
+    f(pix);
+    return;
+  }
+  const int iy = pix / width, ix = pix - iy * width;
+  const int x0 = max(ix - radius, 0), x1 = min(ix + radius, width - 1);
+  const int y0 = max(iy - radius, 0), y1 = min(iy + radius, height - 1);
+  for (int y = y0; y <= y1; y++)
+    for (int x = x0; x <= x1; x++) f(y * width + x);
+}
 
 template <int MODEL, bool F32>
 __global__ void __launch_bounds__(256) lidar_image_project_kernel(const __grid_constant__ LidarImageArgs a) {
@@ -55,7 +72,8 @@ __global__ void __launch_bounds__(256) lidar_image_project_kernel(const __grid_c
   a.sq_dist[i] = sq;
   // :31 `stored < sq_dist` keeps the stored one: the minimum wins (non-negative doubles order like their bit patterns; a point
   // at +inf never beats the initial DBL_MAX, exactly as in the reference)
-  atomicMin(a.zmin + pix, static_cast<unsigned long long>(__double_as_longlong(sq)));
+  const unsigned long long key = static_cast<unsigned long long>(__double_as_longlong(sq));
+  for_each_covered_pixel(pix, a.radius, a.width, a.height, [&](int p) { atomicMin(a.zmin + p, key); });
 }
 
 __global__ void __launch_bounds__(256) lidar_image_winner_kernel(const __grid_constant__ LidarImageArgs a) {
@@ -63,20 +81,23 @@ __global__ void __launch_bounds__(256) lidar_image_winner_kernel(const __grid_co
   if (i >= a.n) return;
   const int pix = a.pix[i];
   if (pix < 0) return;
-  if (static_cast<unsigned long long>(__double_as_longlong(a.sq_dist[i])) == a.zmin[pix]) atomicMax(a.index_image + pix, static_cast<int>(i));  // ties: the last point wins
+  const unsigned long long key = static_cast<unsigned long long>(__double_as_longlong(a.sq_dist[i]));
+  for_each_covered_pixel(pix, a.radius, a.width, a.height, [&](int p) {
+    if (key == a.zmin[p]) atomicMax(a.index_image + p, static_cast<int>(i));  // ties: the last point wins
+  });
 }
 
 template <bool F32>
-__global__ void __launch_bounds__(256) lidar_image_gather_kernel(const __grid_constant__ LidarImageArgs a) {
+__global__ void __launch_bounds__(256) lidar_image_gather_kernel(const void* points, const int* index_image, double* intensity_image, size_t npix) {
   const size_t p = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (p >= static_cast<size_t>(a.width) * a.height) return;
-  const int idx = a.index_image[p];
+  if (p >= npix) return;
+  const int idx = index_image[p];
   double v = 0.0;  // :14
   if (idx >= 0) {
-    if constexpr (F32) v = static_cast<double>(static_cast<const float4*>(a.points)[idx].w);  // lossless by construction of the float4 layout
-    else v = static_cast<const double4*>(a.points)[idx].w;
+    if constexpr (F32) v = static_cast<double>(static_cast<const float4*>(points)[idx].w);  // lossless by construction of the float4 layout
+    else v = static_cast<const double4*>(points)[idx].w;
   }
-  a.intensity_image[p] = v;  // :36
+  intensity_image[p] = v;  // :36
 }
 
 __global__ void lidar_image_init_kernel(unsigned long long* zmin, int* index_image, size_t npix) {
@@ -118,6 +139,38 @@ struct DevBuf {
 };
 }  // namespace
 
+// Passes 1 and 2 for a cloud on the device, enqueued on the legacy stream: d_index_image [H*W] receives the winning point
+// of every pixel (-1: none).  Scratch from the caller: zmin [H*W], pix and sq_dist [max(n, 1)].
+int lidar_index_image_passes(
+  const CameraParams& cam, int width, int height, const double T_camera_lidar[16], const DeviceCloud& cloud, int radius, unsigned long long* zmin, int* pix, double* sq_dist,
+  int* d_index_image) {
+  LidarImageArgs a;
+  std::memset(&a, 0, sizeof(a));
+  a.points = cloud.d_points;
+  a.n = cloud.n;
+  a.width = width, a.height = height;
+  a.radius = radius;
+  a.cos_fov = std::cos(estimate_camera_fov_host(cam, width, height));  // :10-11
+  a.cam = cam;
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 4; c++) a.pose[4 * r + c] = T_camera_lidar[r + 4 * c];
+  a.zmin = zmin;
+  a.pix = pix;
+  a.sq_dist = sq_dist;
+  a.index_image = d_index_image;
+  const size_t npix = static_cast<size_t>(width) * height;
+  lidar_image_init_kernel<<<static_cast<unsigned int>((npix + 255) / 256), 256>>>(a.zmin, a.index_image, npix);
+  VL_CUDA(cudaGetLastError());
+  if (cloud.n > 0) {
+    const unsigned int pt_blocks = static_cast<unsigned int>((cloud.n + 255) / 256);
+    pick_project(cam.model, cloud.f32)<<<pt_blocks, 256>>>(a);
+    VL_CUDA(cudaGetLastError());
+    lidar_image_winner_kernel<<<pt_blocks, 256>>>(a);
+    VL_CUDA(cudaGetLastError());
+  }
+  return VLCAL_OK;
+}
+
 }  // namespace vlcal
 
 using namespace vlcal;
@@ -143,7 +196,6 @@ extern "C" int vlcal_generate_lidar_image(
   }
   if (device < 0) VL_CUDA(cudaGetDevice(&device));
   VL_CUDA(cudaSetDevice(device));
-  const double camera_fov = estimate_camera_fov_host(cam, width, height);  // :10
   std::shared_ptr<DeviceCloud> cloud;
   rc = upload_cloud(device, points_xyzw, intensities, n_points, nullptr, &cloud);
   if (rc != VLCAL_OK) return rc;
@@ -154,34 +206,15 @@ extern "C" int vlcal_generate_lidar_image(
   VL_CUDA(inten.alloc(device, sizeof(double) * npix));
   VL_CUDA(pix.alloc(device, sizeof(int) * std::max<int64_t>(1, n_points)));
   VL_CUDA(sq.alloc(device, sizeof(double) * std::max<int64_t>(1, n_points)));
-  LidarImageArgs a;
-  std::memset(&a, 0, sizeof(a));
-  a.points = cloud->d_points;
-  a.n = n_points;
-  a.width = width, a.height = height;
-  a.cos_fov = std::cos(camera_fov);  // :11
-  a.cam = cam;
-  for (int r = 0; r < 3; r++)
-    for (int c = 0; c < 4; c++) a.pose[4 * r + c] = T_camera_lidar[r + 4 * c];
-  a.zmin = static_cast<unsigned long long*>(zmin.p);
-  a.pix = static_cast<int*>(pix.p);
-  a.sq_dist = static_cast<double*>(sq.p);
-  a.index_image = static_cast<int*>(index.p);
-  a.intensity_image = static_cast<double*>(inten.p);
+  int* d_index = static_cast<int*>(index.p);
+  double* d_inten = static_cast<double*>(inten.p);
+  rc = lidar_index_image_passes(cam, width, height, T_camera_lidar, *cloud, 0, static_cast<unsigned long long*>(zmin.p), static_cast<int*>(pix.p), static_cast<double*>(sq.p), d_index);
+  if (rc != VLCAL_OK) return rc;
   const unsigned int pix_blocks = static_cast<unsigned int>((npix + 255) / 256);
-  lidar_image_init_kernel<<<pix_blocks, 256>>>(a.zmin, a.index_image, npix);
+  if (cloud->f32) lidar_image_gather_kernel<true><<<pix_blocks, 256>>>(cloud->d_points, d_index, d_inten, npix);
+  else lidar_image_gather_kernel<false><<<pix_blocks, 256>>>(cloud->d_points, d_index, d_inten, npix);
   VL_CUDA(cudaGetLastError());
-  if (n_points > 0) {
-    const unsigned int pt_blocks = static_cast<unsigned int>((n_points + 255) / 256);
-    pick_project(cam.model, cloud->f32)<<<pt_blocks, 256>>>(a);
-    VL_CUDA(cudaGetLastError());
-    lidar_image_winner_kernel<<<pt_blocks, 256>>>(a);
-    VL_CUDA(cudaGetLastError());
-  }
-  if (cloud->f32) lidar_image_gather_kernel<true><<<pix_blocks, 256>>>(a);
-  else lidar_image_gather_kernel<false><<<pix_blocks, 256>>>(a);
-  VL_CUDA(cudaGetLastError());
-  VL_CUDA(cudaMemcpy(intensity_image_out, a.intensity_image, sizeof(double) * npix, cudaMemcpyDeviceToHost));
-  VL_CUDA(cudaMemcpy(index_image_out, a.index_image, sizeof(int) * npix, cudaMemcpyDeviceToHost));
+  VL_CUDA(cudaMemcpy(intensity_image_out, d_inten, sizeof(double) * npix, cudaMemcpyDeviceToHost));
+  VL_CUDA(cudaMemcpy(index_image_out, d_index, sizeof(int) * npix, cudaMemcpyDeviceToHost));
   return VLCAL_OK;
 }

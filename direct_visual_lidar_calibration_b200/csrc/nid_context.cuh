@@ -57,6 +57,14 @@ int view_cull_device(
   const CameraParams& cam, int width, int height, double max_fov, bool depth_culling, const DeviceCloud& cloud, const double T[16], cudaStream_t stream,
   std::shared_ptr<DeviceCloud>* culled_out, int32_t* indices_host_out, int64_t* n_kept, bool keep_all = false);
 
+// the z-buffer passes of generate_lidar_image (lidar_image.cu) for a cloud on the device, enqueued on the legacy stream:
+// d_index_image [H*W] receives per pixel the point with the smallest squared range among those that cover it (of equal
+// ones the last; -1: none).  A point covers the pixels within `radius` of its own in x and y (0: the reference's image).
+// Scratch from the caller: zmin [H*W], pix and sq_dist [max(n, 1)].
+int lidar_index_image_passes(
+  const CameraParams& cam, int width, int height, const double T_camera_lidar[16], const DeviceCloud& cloud, int radius, unsigned long long* zmin, int* pix, double* sq_dist,
+  int* d_index_image);
+
 struct ProfileEvents {
   cudaEvent_t start, stop;
   int poses;

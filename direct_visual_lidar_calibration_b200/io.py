@@ -23,18 +23,24 @@ _PLY_TYPES = {
 }
 
 
-def save_ply_binary(path: str, points_xyz, intensities=None) -> None:
-    """Binary little-endian PLY with float x, y, z (+ float intensity), the layout of preprocess.cpp:163-169."""
+def save_ply_binary(path: str, points_xyz, intensities=None, colors=None) -> None:
+    """Binary little-endian PLY with float x, y, z (+ float intensity), the layout of preprocess.cpp:163-169.  colors:
+    (N, 4) RGBA in [0, 1] (the viewer's coloured cloud), appended as uchar red green blue alpha = round(c * 255)."""
     pts = np.asarray(points_xyz, dtype=np.float32).reshape(-1, 3)
     cols = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
     if intensities is not None:
         cols.append(("intensity", "<f4"))
+    if colors is not None:
+        cols += [(name, "u1") for name in ("red", "green", "blue", "alpha")]
     rec = np.empty(pts.shape[0], dtype=cols)
     rec["x"], rec["y"], rec["z"] = pts[:, 0], pts[:, 1], pts[:, 2]
     if intensities is not None:
         rec["intensity"] = np.asarray(intensities, dtype=np.float32).reshape(-1)
+    if colors is not None:
+        rgba = np.rint(np.clip(np.asarray(colors, dtype=np.float64).reshape(-1, 4) * 255.0, 0.0, 255.0)).astype(np.uint8)
+        rec["red"], rec["green"], rec["blue"], rec["alpha"] = rgba.T
     header = ["ply", "format binary_little_endian 1.0", f"element vertex {pts.shape[0]}"]
-    header += [f"property float {name}" for name, _ in cols]
+    header += [f"property {'uchar' if t == 'u1' else 'float'} {name}" for name, t in cols]
     header.append("end_header")
     with open(path, "wb") as f:
         f.write(("\n".join(header) + "\n").encode("ascii"))

@@ -292,6 +292,67 @@ int vlcal_generate_lidar_image(
   double* intensity_image_out,
   int32_t* index_image_out);
 
+/* ---- headless viewer: looking at a calibration (src/viewer.cpp, src/vlcal/common/points_color_updater.cpp) -------------
+ * Both entry points take the camera, the uint8 grayscale image (row_stride bytes per row), the pose and the cloud as
+ * vlcal_generate_lidar_image does, and follow its argument rules (at most 2^31-1 points and pixels; an empty cloud is
+ * legal).  blend_weight in [0, 1] is the weight w of the camera image; a colour is
+ *     gray * w + turbo(intensity) * (1 - w)          gray = pixel / 255.0f, all in float32, 1 - w rounded from double
+ * with turbo(x) = entry clamp(int(float(x) * 255.0), 0, 255) (NaN: 0) of the 256-entry Turbo table / 255.0f.
+ * kernel_ms_out (may be NULL): time of the kernels alone between CUDA events, without uploads and read-back. */
+
+/* the 256 RGB byte triples of the Turbo table the viewer colours intensities with (host data; needs no device) */
+int vlcal_turbo_colormap(uint8_t rgb_out[768]);
+
+/* PointsColorUpdater::update (points_color_updater.cpp:37-61): rgba_out[4 i ..] = colour of point i with alpha 1, or
+ * (0, 0, 0, 0) where the reference skips the point: outside cos(estimate_camera_fov(camera, {width, height}) + 0.5 deg)
+ * -- the viewer's own threshold, looser than the cost's -- or projected outside the image.  Projection, truncation and
+ * bounds test are the NID cost's, decision for decision. */
+int vlcal_colorize_points(
+  int device,
+  int camera_model,
+  const double* intrinsics,
+  int n_intrinsics,
+  const double* distortion,
+  int n_distortion,
+  int width,
+  int height,
+  const uint8_t* image,
+  int row_stride,
+  const double T_camera_lidar[16],
+  const double* points_xyzw,
+  const double* intensities,
+  int64_t n_points,
+  float blend_weight,
+  float* rgba_out, /* n_points x 4 */
+  double* kernel_ms_out);
+
+/* The cloud drawn into the camera image with hidden points removed: per pixel the point with the smallest squared range
+ * wins (of equal ones the last), by the rules and FoV of vlcal_generate_lidar_image, where every point covers the
+ * (2 point_radius + 1)^2 square of pixels around its own, clipped to the image; point_radius in [0, 8], and 0 gives the
+ * index map of vlcal_generate_lidar_image.  bgr_out: H x W x 3 bytes (CV_8UC3), a covered pixel the colour above of its
+ * winner and its own gray value, rounded to nearest, an uncovered pixel its gray value.  index_image_out (may be NULL):
+ * H x W int32, the winner per pixel, -1 where none. */
+int vlcal_render_overlay(
+  int device,
+  int camera_model,
+  const double* intrinsics,
+  int n_intrinsics,
+  const double* distortion,
+  int n_distortion,
+  int width,
+  int height,
+  const uint8_t* image,
+  int row_stride,
+  const double T_camera_lidar[16],
+  const double* points_xyzw,
+  const double* intensities,
+  int64_t n_points,
+  int point_radius,
+  float blend_weight,
+  uint8_t* bgr_out,
+  int32_t* index_image_out,
+  double* kernel_ms_out);
+
 /* ---- solver surface ------------------------------------------------------------------ */
 
 /* how vlcal_estimate_pose_nelder_mead* / vlcal_calibrate_nelder_mead iterate (process-wide):
