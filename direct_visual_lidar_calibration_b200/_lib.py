@@ -153,7 +153,6 @@ def load_library():
     L.vlcal_nid_get_profile_delta.argtypes = [vp, C.POINTER(C.c_int64)]
     L.vlcal_nid_debug_solve_stamps.argtypes = [vp, C.c_int, C.POINTER(C.c_uint64), ip]
     L.vlcal_nid_debug_block_times.argtypes = [vp, C.c_int, C.POINTER(C.c_uint64), ip]
-    L.vlcal_nid_debug_tma_stats.argtypes = [vp, C.POINTER(C.c_uint64)]
     L.vlcal_nid_evaluate_bspline.argtypes = [vp, dp, C.c_int, dp, vp, vp]
     L.vlcal_nid_evaluate_bspline_grad.argtypes = [vp, dp, C.c_int, dp, dp, vp]
     L.vlcal_nid_num_points.argtypes = [vp]

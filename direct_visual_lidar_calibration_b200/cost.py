@@ -170,12 +170,6 @@ class CostCalculatorNID:
         _lib.check(self._L.vlcal_nid_debug_last_points_per_lane(self._ctx, C.byref(k)))
         return int(k.value)
 
-    def tma_stats(self):
-        """(gathers served by the TMA-staged shared-memory window, gathers that escaped to global memory) of the last persistent solve (VLCAL_PK_TMA=1)."""
-        buf = (C.c_uint64 * 2)()
-        _lib.check(self._L.vlcal_nid_debug_tma_stats(self._ctx, buf))
-        return int(buf[0]), int(buf[1])
-
     def block_times(self, capacity: int = 2048):
         """(n_blocks, 4) uint64 ns stamps of one batch of the last stamped persistent solve: enter, zeroed, main loop done, arrived."""
         buf = (C.c_uint64 * (4 * capacity))()

@@ -82,7 +82,6 @@ struct LeanVerdict {
   bool accept;     // the reference certainly counts this point at pixel `idx`
   bool uncertain;  // within the error bound of a decision edge: ask the exact path
   int idx;         // iy * W + ix, meaningful when accept
-  int ixb, iyb;    // ix + LEAN_MAGIC_BITS, iy + LEAN_MAGIC_BITS (the rounded coordinates as they come out of the magic add)
   float up, vp;    // the fp32 projection minus 0.5, and
   float hx, hy;    // 0.5 - E: what the verify kernel needs to measure how much of the bound the fp32 error uses
 };
@@ -117,7 +116,6 @@ VL_HD LeanVerdict lean_tail(const LeanCam& c, int width, float up, float vp, flo
   // truncation toward zero: rint(u') == -1 (u in (-1, 0)) is column 0
   const int ixb = max(LEAN_F2I(tx), LEAN_MAGIC_BITS), iyb = max(LEAN_F2I(ty), LEAN_MAGIC_BITS);
   v.idx = iyb * width + ixb - c.idx_bias;
-  v.ixb = ixb, v.iyb = iyb;
   v.up = up, v.vp = vp, v.hx = hx, v.hy = hy;
   return v;
 }

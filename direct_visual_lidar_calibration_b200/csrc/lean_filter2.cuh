@@ -47,7 +47,7 @@ __device__ __forceinline__ F2 f2_rsqrt(F2 a) {
 // what the hot loop needs of a verdict (the verify kernel also reads the projection and the half-widths)
 struct LeanVerdict2 {
   bool accept[2], uncertain[2];
-  int idx[2], ixb[2], iyb[2];
+  int idx[2];
   float up[2], vp[2], hx[2], hy[2];
 };
 
@@ -73,7 +73,6 @@ __device__ __forceinline__ LeanVerdict2 lean_tail2(const LeanCam& c, int width, 
     v.uncertain[h] = !cert & !rej[h];
     const int ixb = max(__float_as_int(txs[h]), LEAN_MAGIC_BITS), iyb = max(__float_as_int(tys[h]), LEAN_MAGIC_BITS);
     v.idx[h] = iyb * width + ixb - c.idx_bias;
-    v.ixb[h] = ixb, v.iyb[h] = iyb;
     v.hx[h] = hxs[h], v.hy[h] = hys[h];
   }
   return v;

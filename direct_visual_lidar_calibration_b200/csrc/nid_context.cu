@@ -320,21 +320,14 @@ static std::mutex g_geom_mu;
 // keyed by device too: function attributes (the dynamic shared memory opt-in) and occupancy are per device / context
 static std::map<std::tuple<int, const void*, size_t>, int> g_occupancy_cache;
 
-static int hist_copies_cap() {
-  // warp-private copies bought nothing measurable over a couple of shared ones in a shared-atomic microbenchmark
-  // (tools/microbench.cu), but every copy is zeroed and merged by every block on every launch; VLCAL_HIST_COPIES overrides for A/B
-  static const int cap = [] {
-    const char* e = std::getenv("VLCAL_HIST_COPIES");
-    const int v = e ? std::atoi(e) : 2;
-    return std::max(1, std::min(v, NID_THREADS / 32));
-  }();
-  return cap;
-}
+// warp-private copies bought nothing measurable over a couple of shared ones in a shared-atomic microbenchmark
+// (tools/microbench.cu), but every copy is zeroed and merged by every block on every launch
+constexpr int HIST_COPIES_CAP = 2;
 
 static int launch_geometry(int device, NidKernel kernel, int n_poses, int nb, int bins, LaunchGeom* g) {
   const size_t per_copy = static_cast<size_t>(n_poses) * nb * sizeof(int);
   int copies = static_cast<int>(NID_SMEM_TARGET / per_copy);
-  copies = std::max(1, std::min(copies, hist_copies_cap()));
+  copies = std::max(1, std::min(copies, HIST_COPIES_CAP));
   g->copies = copies;
   g->smem = per_copy * copies;
   // room for nid_finalize to split one pose over several warps: 8 pose slots x (nb doubles + 2*bins ints)
@@ -991,12 +984,6 @@ int vlcal_nid_debug_solve_stamps(vlcal_nid_ctx* ctx, int capacity, uint64_t* sta
   return VLCAL_OK;
 }
 
-int vlcal_nid_debug_tma_stats(vlcal_nid_ctx* ctx, uint64_t stats[2]) {
-  if (!ctx || !stats) return VLCAL_ERR_INVALID_ARGUMENT;
-  stats[0] = ctx->pk_tma_stats[0], stats[1] = ctx->pk_tma_stats[1];
-  return VLCAL_OK;
-}
-
 int vlcal_nid_debug_last_points_per_lane(const vlcal_nid_ctx* ctx, int* k_out) {
   if (!ctx || !k_out) return VLCAL_ERR_INVALID_ARGUMENT;
   *k_out = ctx->pk_last_kpt;
@@ -1187,7 +1174,7 @@ static int debug_filter_check(vlcal_nid_ctx* ctx, const double* T_camera_lidar, 
     set_last_error("the fp32 filter is not enabled for this context (camera model / FoV / point layout)");
     return VLCAL_ERR_UNSUPPORTED;
   }
-  if (delta && (ctx->cam.model != CAM_EQUIRECTANGULAR || !ctx->lean.enabled || !PK_PACKED_FP32)) {
+  if (delta && (ctx->cam.model != CAM_EQUIRECTANGULAR || !ctx->lean.enabled)) {
     set_last_error("the delta step exists for the packed equirectangular classifier only");
     return VLCAL_ERR_UNSUPPORTED;
   }

@@ -141,7 +141,6 @@ struct vlcal_nid_ctx {
   int pk_chunk = 8;  // poses per pass of the persistent kernel's pose-list mode (vlcal_nid_set_poses_per_pass)
   int pk_stamps_cap = 0;
   std::vector<unsigned long long> pk_stamps;
-  unsigned long long pk_tma_stats[2] = {0, 0};  // TMA variant, last solve: gathers served by the staged window / escaped to global memory
   std::vector<unsigned long long> pk_block_times;  // [grid][4] of one batch (vlcal_nid_debug_block_times)
   int pk_last_kpt = 0;  // points per lane of the instance the last persistent launch on this context ran (0: none yet)
 

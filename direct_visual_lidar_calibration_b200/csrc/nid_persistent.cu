@@ -4,8 +4,6 @@
 // (CostCalculatorNID::calculate per pose, src/vlcal/calib/cost_calculator_nid.cpp:21-67) in ONE launch.
 #include "nid_persistent.cuh"
 
-#include <cuda.h>  // CUtensorMap + cuTensorMapEncodeTiled's signature (resolved through cudaGetDriverEntryPoint: no libcuda link)
-
 #include <algorithm>
 #include <atomic>
 #include <chrono>
@@ -25,85 +23,32 @@ namespace vlcal {
 using PkKernel = void (*)(const PkArgs);
 
 // points per lane and tile: 2 or 4 for the light models, 2 for the ones that carry transcendental calls (more live state
-// per point); atom: histogram-increment form (nid_persistent.cuh)
-#ifndef PK_K4_ALL
-#define PK_K4_ALL 0  // A/B builds: also instantiate 4 points per lane for the models whose classifier is register-heavy
-#endif
+// per point)
 template <int MODEL>
-static PkKernel pk_pick_ka(int k, int atom) {
+static PkKernel pk_pick_k(int k) {
   constexpr bool heavy = MODEL == CAM_FISHEYE || MODEL == CAM_EQUIRECTANGULAR || MODEL == CAM_ATAN;
-  if constexpr (!heavy || PK_K4_ALL) {
-    if (k == 4) return atom ? nid_persistent_kernel<MODEL, 4, 1> : nid_persistent_kernel<MODEL, 4, 0>;
+  if constexpr (!heavy) {
+    if (k == 4) return nid_persistent_kernel<MODEL, 4>;
   }
-  return atom ? nid_persistent_kernel<MODEL, 2, 1> : nid_persistent_kernel<MODEL, 2, 0>;
+  return nid_persistent_kernel<MODEL, 2>;
 }
 
-// the points per lane of the kernel pk_pick_ka returns for a requested k
+// the points per lane of the kernel pk_pick_k returns for a requested k
 static int pk_kernel_k(int model, int k) {
   const bool heavy = model == CAM_FISHEYE || model == CAM_EQUIRECTANGULAR || model == CAM_ATAN;
-  return k == 4 && (!heavy || PK_K4_ALL) ? 4 : 2;
-}
-
-static int pk_tma_requested() {
-  static const int v = [] {
-    const char* e = std::getenv("VLCAL_PK_TMA");
-    return e ? std::atoi(e) : 0;  // A/B: the staged window did not pay for its index arithmetic -> off
-  }();
-  return v;
-}
-
-// TMA variant: instantiated for the C2 shape only (plumb_bob, 2 points per lane, merged increments)
-static PkKernel pk_pick_tma(int model, int k) {
-  if (model == CAM_PLUMB_BOB && k == 2) return nid_persistent_kernel<CAM_PLUMB_BOB, 2, 0, true>;
-  return nullptr;
-}
-
-// tensor map of an image-bin plane: u8, W x H, tight rows, box 256 x 1, out-of-bounds bytes read as zero
-static int pk_make_tensor_map(const uint8_t* img, int width, int height, PkTensorMap* out) {
-  using EncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  static EncodeFn encode = [] {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || qres != cudaDriverEntryPointSuccess) fn = nullptr;
-    cudaGetLastError();
-    return reinterpret_cast<EncodeFn>(fn);
-  }();
-  if (!encode) {
-    set_last_error("cuTensorMapEncodeTiled is not available from this driver");
-    return VLCAL_ERR_UNSUPPORTED;
-  }
-  static_assert(sizeof(CUtensorMap) == sizeof(PkTensorMap), "CUtensorMap is 128 bytes");
-  CUtensorMap m;
-  const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(width), static_cast<cuuint64_t>(height)};
-  const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(width)};  // bytes between rows (multiple of 16: checked by the caller)
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(PK_TMA_BOX_W), 1u};
-  const cuuint32_t estride[2] = {1u, 1u};
-  const CUresult r = encode(&m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<uint8_t*>(img), gdim, gstride, box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                            CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error("cuTensorMapEncodeTiled failed with code " + std::to_string(static_cast<int>(r)));
-    return VLCAL_ERR_CUDA;
-  }
-  std::memcpy(out, &m, sizeof(m));
-  return VLCAL_OK;
+  return k == 4 && !heavy ? 4 : 2;
 }
 
 // delta: the launch may carry equirectangular batches of nearby poses (the instance with the delta step, K = 2)
 static PkKernel pk_pick(int model, int k, bool delta = false) {
-  static const int atom = [] {
-    const char* e = std::getenv("VLCAL_PK_ATOM");
-    return e ? (std::atoi(e) != 0 ? 1 : 0) : 0;
-  }();
-  if (PK_DELTA_POSES && delta && model == CAM_EQUIRECTANGULAR && pk_kernel_k(model, k) == 2)
-    return atom ? nid_persistent_kernel<CAM_EQUIRECTANGULAR, 2, 1, false, true> : nid_persistent_kernel<CAM_EQUIRECTANGULAR, 2, 0, false, true>;
+  if (PK_DELTA_POSES && delta && model == CAM_EQUIRECTANGULAR && pk_kernel_k(model, k) == 2) return nid_persistent_kernel<CAM_EQUIRECTANGULAR, 2, true>;
   switch (model) {
-    case CAM_PLUMB_BOB: return pk_pick_ka<CAM_PLUMB_BOB>(k, atom);
-    case CAM_FISHEYE: return pk_pick_ka<CAM_FISHEYE>(k, atom);
-    case CAM_ATAN: return pk_pick_ka<CAM_ATAN>(k, atom);
-    case CAM_OMNIDIR: return pk_pick_ka<CAM_OMNIDIR>(k, atom);
-    case CAM_EQUIRECTANGULAR: return pk_pick_ka<CAM_EQUIRECTANGULAR>(k, atom);
-    case CAM_RATIONAL_POLYNOMIAL: return pk_pick_ka<CAM_RATIONAL_POLYNOMIAL>(k, atom);
+    case CAM_PLUMB_BOB: return pk_pick_k<CAM_PLUMB_BOB>(k);
+    case CAM_FISHEYE: return pk_pick_k<CAM_FISHEYE>(k);
+    case CAM_ATAN: return pk_pick_k<CAM_ATAN>(k);
+    case CAM_OMNIDIR: return pk_pick_k<CAM_OMNIDIR>(k);
+    case CAM_EQUIRECTANGULAR: return pk_pick_k<CAM_EQUIRECTANGULAR>(k);
+    case CAM_RATIONAL_POLYNOMIAL: return pk_pick_k<CAM_RATIONAL_POLYNOMIAL>(k);
     default: return nullptr;
   }
 }
@@ -118,10 +63,10 @@ struct PkGeom {
 static std::mutex g_pk_mu;
 static std::map<std::tuple<int, const void*, size_t>, int> g_pk_occupancy;
 
-// Dynamic shared memory of one block: the histogram copies (whose space the finalizer reuses as staging), then either
-// the TMA variant's image window or the warps' tile rings.  At 16 bins and K = 2: 48 KB of copies + 24 warps x 2 slots
-// x 1 KB of rings = 96 KB, next to ~16 KB of static PkShared -- within the 227 KB a block may opt in to on an H100.
-static int pk_geometry(int device, int num_sms, PkKernel kernel, int nb, int kpt, PkGeom* g, bool tma = false) {
+// Dynamic shared memory of one block: the histogram copies (whose space the finalizer reuses as staging), then the warps'
+// tile rings.  At 16 bins and K = 2: 48 KB of copies + 24 warps x 2 slots x 1 KB of rings = 96 KB, next to ~16 KB of
+// static PkShared -- within the 227 KB a block may opt in to on an H100.
+static int pk_geometry(int device, int num_sms, PkKernel kernel, int nb, int kpt, PkGeom* g) {
   // histogram copies for 8 poses (the initial simplex of a 6-D solve is 7) -- two copies while they fit 64 KB
   const size_t per_copy = static_cast<size_t>(PK_MAX_POSES) * nb * sizeof(int);
   g->copies = static_cast<int>(std::max<size_t>(1, std::min<size_t>(PK_WARPS / 4, (64 * 1024) / per_copy)));  // one copy per four warps
@@ -129,8 +74,7 @@ static int pk_geometry(int device, int num_sms, PkKernel kernel, int nb, int kpt
   g->smem = std::max(per_copy * g->copies, scratch);
   const size_t tail = (g->smem + 127) & ~static_cast<size_t>(127);
   g->ring_off = static_cast<unsigned int>(tail);
-  if (tma) g->smem = tail + PK_TMA_BYTES;
-  else if (PK_TILE_RING) g->smem = tail + pk_ring_bytes(kpt);
+  g->smem = tail + pk_ring_bytes(kpt);
   std::lock_guard<std::mutex> lock(g_pk_mu);
   const auto key = std::make_tuple(device, reinterpret_cast<const void*>(kernel), g->smem);
   auto it = g_pk_occupancy.find(key);
@@ -165,11 +109,9 @@ static unsigned long long pk_timeout_ns() {
 
 // Points per lane and tile (K).  Tiles are dealt to the warps round-robin, so K = 4 (128-point tiles) needs a cloud large
 // enough for several tiles per warp to stay balanced -- and there the lighter register footprint of K = 2 (768 threads per
-// SM without spills in the pose loop, one packed register pair per coordinate) measured faster anyway.  K = 4 remains as variant 3 / VLCAL_PK_KPT=4 for A/B runs.
-static int pk_points_per_lane(const vlcal_nid_ctx* ctx, long long /*total_points*/) {
-  if (const char* e = std::getenv("VLCAL_PK_KPT")) return std::atoi(e) == 4 ? 4 : 2;
-  return ctx->variant == 3 ? 4 : 2;
-}
+// SM without spills in the pose loop, one packed register pair per coordinate) measured faster anyway.  K = 4 remains as
+// variant 3.
+static int pk_points_per_lane(const vlcal_nid_ctx* ctx) { return ctx->variant == 3 ? 4 : 2; }
 
 bool pk_supported(vlcal_nid_ctx* const* ctxs, int n_ctxs) {
   if (n_ctxs < 1 || n_ctxs > PK_MAX_BAGS) return false;
@@ -198,7 +140,7 @@ struct PinBuf {
 
 // device scratch of one launch, one allocation, zeroed by one memset
 struct PkScratchLayout {
-  size_t ghist, gmarg, arrive, fin_done, tile_next, abort_flag, seq, tma_stats, delta_stats, box, solve, total;
+  size_t ghist, gmarg, arrive, fin_done, tile_next, abort_flag, seq, delta_stats, box, solve, total;
   PkScratchLayout(int n_bags, int nb) {
     size_t o = 0;
     auto take = [&](size_t bytes) {
@@ -213,7 +155,6 @@ struct PkScratchLayout {
     tile_next = take(sizeof(unsigned int) * 2 * PK_MAX_BAGS);
     abort_flag = take(sizeof(unsigned int));
     seq = take(sizeof(unsigned long long));
-    tma_stats = take(sizeof(unsigned long long) * 2);
     delta_stats = take(sizeof(unsigned long long) * 4);
     box = take(sizeof(PkMailbox));
     solve = take(sizeof(PkSolve));
@@ -277,17 +218,11 @@ int pk_solve(
   vlcal_nm_result* nm_result) {
   vlcal_nid_ctx* c0 = ctxs[0];
   VL_CUDA(cudaSetDevice(c0->device));
-  long long total_points = 0;
-  for (int i = 0; i < n_ctxs; i++) total_points += ctxs[i]->cloud->n;
-  const int kpt = pk_points_per_lane(c0, total_points);
-  PkKernel kernel = pk_pick(c0->cam.model, kpt, true);  // Nelder-Mead batches close in as the simplex shrinks
-  // TMA variant (A/B): image windows staged in shared memory; needs 16-byte row pitches and 128-byte aligned histogram copies
-  const size_t hist_bytes = static_cast<size_t>(std::max<size_t>(1, std::min<size_t>(PK_WARPS / 4, (64 * 1024) / (static_cast<size_t>(PK_MAX_POSES) * c0->bins * c0->bins * 4)))) * PK_MAX_POSES * c0->bins * c0->bins * 4;
-  const bool use_tma = pk_tma_requested() != 0 && pk_pick_tma(c0->cam.model, kpt) != nullptr && c0->image->width % 16 == 0 && hist_bytes % 128 == 0;
-  if (use_tma) kernel = pk_pick_tma(c0->cam.model, kpt);
+  const int kpt = pk_points_per_lane(c0);
+  const PkKernel kernel = pk_pick(c0->cam.model, kpt, true);  // Nelder-Mead batches close in as the simplex shrinks
   PkGeom g;
   {
-    const int rc = pk_geometry(c0->device, c0->num_sms, kernel, c0->bins * c0->bins, pk_kernel_k(c0->cam.model, kpt), &g, use_tma);
+    const int rc = pk_geometry(c0->device, c0->num_sms, kernel, c0->bins * c0->bins, pk_kernel_k(c0->cam.model, kpt), &g);
     if (rc != VLCAL_OK) return rc;
   }
   const int grid = pk_grid_size(g, ctxs, n_ctxs);
@@ -334,13 +269,6 @@ int pk_solve(
   PkArgs a;
   pk_fill_common(a, ctxs, n_ctxs, g, grid, sp, L);
   a.solve = reinterpret_cast<const PkSolve*>(sp + L.solve);
-  if (use_tma) {
-    for (int i = 0; i < n_ctxs; i++) {
-      const int rc = pk_make_tensor_map(ctxs[i]->d_bin_image, c0->image->width, c0->image->height, &a.tmap[i]);
-      if (rc != VLCAL_OK) return rc;
-    }
-    a.tma_stats = reinterpret_cast<unsigned long long*>(sp + L.tma_stats);
-  }
   a.result_host = h_result;
   a.trace_host = h_trace;
   a.trace_cap = trace_cap;
@@ -416,7 +344,6 @@ int pk_solve(
   }
   // scratch goes back to the pool: the kernel has published its last word, nothing else is enqueued on it
   VL_CUDA(cudaStreamSynchronize(c0->stream));
-  if (use_tma) VL_CUDA(cudaMemcpy(c0->pk_tma_stats, sp + L.tma_stats, sizeof(c0->pk_tma_stats), cudaMemcpyDeviceToHost));
   unsigned long long delta_stats[4];
   VL_CUDA(cudaMemcpy(delta_stats, sp + L.delta_stats, sizeof(delta_stats), cudaMemcpyDeviceToHost));
 
@@ -465,9 +392,7 @@ int pk_solve(
 int pk_score_poses(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_colmajor, int n_poses, double* nid_out, int32_t* hist_out) {
   vlcal_nid_ctx* c0 = ctxs[0];
   VL_CUDA(cudaSetDevice(c0->device));
-  long long total_points = 0;
-  for (int i = 0; i < n_ctxs; i++) total_points += ctxs[i]->cloud->n;
-  const int kpt = pk_points_per_lane(c0, total_points);
+  const int kpt = pk_points_per_lane(c0);
   // the instance with the delta step only when some chunk of the list lies within its gate (the kernel checks every
   // chunk again); widely spread lists and one-pose chunks keep the plain instance
   bool delta = false;

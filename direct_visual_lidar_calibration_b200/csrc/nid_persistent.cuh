@@ -29,7 +29,6 @@
 // Several bags per GPU: the grid is partitioned over the bags in proportion to their sizes (one tail for all bags).
 #pragma once
 
-#include <climits>
 #include <cstdint>
 
 #include "exact_classify.cuh"
@@ -39,14 +38,11 @@
 
 namespace vlcal {
 
-// Launch shape: ONE block of 768 threads per SM (24 warps, <= 85 registers).  Three blocks of 256 threads (A/B build,
-// `make alt ALTFLAGS="-DPK_THREADS_CFG=256 -DPK_MIN_BLOCKS=3"`) hold the same 24 warps, but the warp scheduler prefers higher warp slots, so the three blocks of an SM
-// finish their equal slices at different times and every Nelder-Mead batch waits for the slowest; one block also merges
-// once instead of three times and arrives once.
-#ifndef PK_THREADS_CFG
-#define PK_THREADS_CFG 768
-#endif
-constexpr int PK_THREADS = PK_THREADS_CFG;
+// Launch shape: ONE block of 768 threads per SM (24 warps, <= 85 registers: 768 threads fill the register file).  Three
+// blocks of 256 threads hold the same 24 warps, but the warp scheduler prefers higher warp slots, so the three blocks of
+// an SM finish their equal slices at different times and every Nelder-Mead batch waits for the slowest; one block also
+// merges once instead of three times and arrives once.
+constexpr int PK_THREADS = 768;
 constexpr int PK_WARPS = PK_THREADS / 32;
 constexpr int PK_MAX_POSES = 8;
 constexpr int PK_MAX_BAGS = 8;
@@ -56,39 +52,16 @@ constexpr int PK_MAX_BINS = 32;  // nb <= 1024
 constexpr int PK_MARG_STRIDE = 2 * PK_MAX_BINS + 32;  // ints per (bag, pose) record of PkArgs::gmarg
 constexpr int PK_STAMP_SLOTS = 8;
 constexpr unsigned int PK_TILE_ROWS = 4;
-// TMA variant (A/B, VLCAL_PK_TMA=1): the block's window of the image-bin plane staged in shared memory once per solve
-constexpr int PK_TMA_BYTES = 48 * 1024;  // shared memory of the window
-constexpr int PK_TMA_BOX_W = 256;        // one TMA box = 256 x 1 bytes of a row (boxes of a row are contiguous in shared memory)
-constexpr int PK_TMA_HALO = 12;          // pixels around the bounding box of the block's points at the start pose
-struct alignas(64) PkTensorMap {         // a CUtensorMap (cuTensorMapEncodeTiled), opaque here
-  unsigned long long opaque[16];
-};
-#ifndef PK_PACKED_FP32
-#define PK_PACKED_FP32 1  // classify two points per lane, interleaved (lean_filter2.cuh); 0: scalar classifier (A/B build)
-#endif
-#ifndef PK_DIAG_STAMPS
-#define PK_DIAG_STAMPS 0  // diagnostic build: stamp 3 moves behind the two-ahead zeroing, stamp 5 to the finalizer's inner barrier
-#endif
-#ifndef PK_MIN_BLOCKS
-#define PK_MIN_BLOCKS 1  // blocks per SM the register allocation must allow (768 threads x 85 registers fill the register file)
-#endif
-// Tile ring (interleaved split, not the TMA variant): every warp streams its tiles through PK_RING_SLOTS shared-memory
-// slots filled by per-lane 16-byte cp.async copies; 0: the next tile's rows are prefetched into registers (A/B build)
-#ifndef PK_TILE_RING
-#define PK_TILE_RING 1
-#endif
-#ifndef PK_RING_SLOTS
-#define PK_RING_SLOTS 2  // PK_RING_SLOTS - 1 tiles in flight; every slot more takes 24 KB of the SM's L1 for shared memory
-#endif
-constexpr int PK_RING = PK_RING_SLOTS;
+// Tile ring: every warp streams its tiles through PK_RING shared-memory slots filled by per-lane 16-byte cp.async copies.
+// PK_RING - 1 tiles are in flight; every slot more takes 24 KB of the SM's L1 for shared memory.
+constexpr int PK_RING = 2;
 // Equirectangular batches of nearby poses: poses 1..P-1 as first-order updates from pose 0 (classify_lean2_delta);
-// 0: every pose through the plain classifier (A/B build)
+// 0: every pose through the plain classifier (A/B build, `make alt`)
 #ifndef PK_DELTA_POSES
 #define PK_DELTA_POSES 1
 #endif
-static_assert(PK_RING >= 2 && PK_RING <= 8, "PK_RING_SLOTS: 2..8 tile slots per warp");
 // dynamic shared memory of the block's tile rings: PK_WARPS x PK_RING slots of one 32*k-point tile (float4 rows)
-__host__ __device__ constexpr unsigned int pk_ring_bytes(int k) { return PK_TILE_RING ? static_cast<unsigned int>(PK_WARPS * PK_RING * 32 * k * 16) : 0u; }
+__host__ __device__ constexpr unsigned int pk_ring_bytes(int k) { return static_cast<unsigned int>(PK_WARPS * PK_RING * 32 * k * 16); }
 
 // score exchange: every double travels as two 8-byte words {32 data bits | 32-bit sequence tag} (an aligned 8-byte store
 // is never torn, so the data is its own arrival flag).  w[slot][(rank * n_bags + bag) * 8 + pose][lo, hi]
@@ -117,8 +90,10 @@ struct PkResult {
   int pad_;
 };
 
-struct PkArgs {
-  PkTensorMap tmap[PK_MAX_BAGS];  // TMA variant: tensor map of each bag's image-bin plane (u8, W x H, box 256 x 1)
+// 64-byte aligned: with the kernel's parameter block at 8-byte alignment, ptxas allocates registers differently and the
+// plumb_bob K = 4 instance spills 28 bytes instead of 16 (and reloads 148 instead of 20), omnidir K = 2 reloads 120
+// bytes instead of 100
+struct alignas(64) PkArgs {
   // camera + image geometry (shared by all bags of the launch: one camera, equal image sizes)
   int width, height, bins, nb;
   double cos_fov;
@@ -154,7 +129,6 @@ struct PkArgs {
   unsigned long long done_seq;
   unsigned long long* stamps;       // optional [cap][PK_STAMP_SLOTS] globaltimer stamps per batch
   int stamps_cap;
-  unsigned long long* tma_stats;    // TMA variant: [0] gathers served from the shared-memory window, [1] gathers that escaped it
   // [4]: passes (batches / chunks) that took the delta step and their poses (block 0), point-poses deferred to the exact
   // path in the other passes and in those passes (every block)
   unsigned long long* delta_stats;
@@ -180,10 +154,6 @@ struct PkShared {
   unsigned long long poses_scored;
   unsigned long long seq_base;
   int s_cnt[PK_WARPS];
-  // TMA variant: the staged window [box_h][box_w] of the image-bin plane (origin biased like LeanVerdict::ixb / iyb)
-  alignas(8) unsigned long long tma_bar;
-  int bb_min_x, bb_max_x, bb_min_y, bb_max_y;
-  int box_x0b, box_y0b, box_w, box_h;
   unsigned int q_idx[PK_WARPS][PK_QUEUE];
   unsigned char q_pose[PK_WARPS][PK_QUEUE];
   int q_cnt[PK_WARPS];  // fill count of each warp's queue
@@ -199,13 +169,9 @@ __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int* p) {
   return v;
 }
 
-// histogram increment, two forms (A/B, VLCAL_PK_ATOM):
-//   ATOM == 0: `if (counted) atomicAdd(p, 1)` -- ptxas emits BSSY / BRA / ATOMS.POPC.INC / BSYNC (lanes of a warp that hit
-//              the same bin are merged by the hardware; predication is not available for this form, hence the branch);
-//   ATOM == 1: unconditional red.shared.add of a 0 / 1 register -- one ATOMS.ADD, no branch, same-bin lanes serialise.
-__device__ __forceinline__ void red_shared_add(unsigned int smem_addr, int inc) {
-  asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(smem_addr), "r"(inc) : "memory");
-}
+// histogram increment, under `if (counted)`: ptxas emits BSSY / BRA / ATOMS.POPC.INC / BSYNC (lanes of a warp that hit the
+// same bin are merged by the hardware; predication is not available for this form, hence the branch).  An unconditional
+// red.shared.add of a 0 / 1 register (one ATOMS.ADD, no branch, but same-bin lanes serialise) measured slower.
 __device__ __forceinline__ void red_shared_inc(unsigned int smem_addr) {
   asm volatile("red.shared.add.u32 [%0], 1;" ::"r"(smem_addr) : "memory");
 }
@@ -214,22 +180,6 @@ __device__ __forceinline__ void red_shared_inc(unsigned int smem_addr) {
 __device__ __forceinline__ int ldg_u8_or_neg(bool pred, const uint8_t* p) {
   int v;
   asm("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %1, 0;\n\tmov.u32 %0, -1;\n\t@q ld.global.nc.u8 %0, [%2];\n\t}" : "=r"(v) : "r"(static_cast<int>(pred)), "l"(p));
-  return v;
-}
-
-__device__ __forceinline__ int ldg_u8_or_zero(bool pred, const uint8_t* p) {
-  int v;
-  asm("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %1, 0;\n\tmov.u32 %0, 0;\n\t@q ld.global.nc.u8 %0, [%2];\n\t}" : "=r"(v) : "r"(static_cast<int>(pred)), "l"(p));
-  return v;
-}
-
-// TMA variant: the image bin from the staged window (shared memory) when the pixel lies inside it, from global memory
-// otherwise; `neg` = -1 (ATOM == 0: the sign is the "counted" flag) or 0
-__device__ __forceinline__ int gather_u8_window(bool in_window, bool outside, unsigned int smem_addr, const uint8_t* p, int neg) {
-  int v;
-  asm("{\n\t.reg .pred q, r;\n\tsetp.ne.b32 q, %1, 0;\n\tsetp.ne.b32 r, %2, 0;\n\tmov.u32 %0, %5;\n\t@q ld.shared.u8 %0, [%3];\n\t@r ld.global.nc.u8 %0, [%4];\n\t}"
-      : "=r"(v)
-      : "r"(static_cast<int>(in_window)), "r"(static_cast<int>(outside)), "r"(smem_addr), "l"(p), "r"(neg));
   return v;
 }
 
@@ -682,7 +632,7 @@ static __device__ __noinline__ double pk_block_nid(PkShared& sh, int* __restrict
 __host__ __device__ constexpr int pk_fin_item_bytes(int nb, int bins) { return 8 * (nb + 2 * bins); }
 
 static __device__ __noinline__ void pk_block_nid_items(const int* __restrict__ gbuf, const int* __restrict__ mbuf, int first, int count, int n_poses, int nb, int bins, void* scratch,
-                                                       double* out, unsigned long long* diag_stamp) {
+                                                       double* out) {
   double* s_term = static_cast<double*>(scratch);  // [count][nb + 2*bins]: joint terms, image-marginal terms, lidar-marginal terms
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const int per_item = nb + 2 * bins;
@@ -714,7 +664,6 @@ static __device__ __noinline__ void pk_block_nid_items(const int* __restrict__ g
     }
   }
   __syncthreads();
-  if (diag_stamp && t == 0) *diag_stamp = global_ns();
   if (warp < count) {
     const double* tj = s_term + static_cast<size_t>(warp) * per_item;
     double t_rs = 0.0, t_r = 0.0, t_s = 0.0;
@@ -780,11 +729,6 @@ __device__ __forceinline__ int atoms_add(unsigned int addr, int v) {
 
 struct PkWarp {
   unsigned int hist_addr;  // shared-memory byte address of this warp's histogram copy [P][nb]
-  // TMA variant
-  unsigned int win_addr;   // shared-memory byte address of the staged image window
-  int win_x0b, win_y0b;
-  unsigned int win_w, win_h;
-  unsigned int n_window, n_escaped;
   // the warp's queue of deferred (point, pose) pairs, as shared-window byte addresses (generic pointers would turn the pushes into
   // generic stores / generic atomics)
   unsigned int q_idx;   // unsigned int [PK_QUEUE]
@@ -827,7 +771,7 @@ __device__ __forceinline__ void pk_drain32(const PkArgs& a, const PkShared& sh, 
 // pose p stay in flight while pose p+1 is classified and are consumed by the histogram increments one iteration later.
 // PARTIAL: the tile may reach past `end` (only the single-row tiles at the end of a warp's slice).
 // DPOSE: the kernel instance carries the equirectangular delta step (nid_persistent_kernel).
-template <int MODEL, int K, bool PARTIAL, int ATOM, bool TMA, bool DPOSE = false>
+template <int MODEL, int K, bool PARTIAL, bool DPOSE = false>
 __device__ __forceinline__ void pk_tile(const PkArgs& a, const PkShared& sh, const PkBagRegs& B, int n_poses, PkWarp& w, unsigned int tile, unsigned int end, const float4 (&q)[K]) {
   float px[K], py[K], pz[K], dl[K];
   unsigned int lb[K];
@@ -839,7 +783,7 @@ __device__ __forceinline__ void pk_tile(const PkArgs& a, const PkShared& sh, con
     dl[j] = (5.25f * F32_U) * (fabsf(q[j].x) + fabsf(q[j].y) + fabsf(q[j].z) + tmax);
     lb[j] = w.hist_addr + 4u * static_cast<unsigned int>(lidar_bin_of(q[j].w, a.bins) * a.bins);
   }
-  constexpr bool PACKED = PK_PACKED_FP32 && !PARTIAL && (K % 2 == 0) && LeanPacked<MODEL>::value;
+  constexpr bool PACKED = !PARTIAL && (K % 2 == 0) && LeanPacked<MODEL>::value;
   F2 X2[(K + 1) / 2], Y2[(K + 1) / 2], Z2[(K + 1) / 2], D2[(K + 1) / 2];
   if constexpr (PACKED) {
 #pragma unroll
@@ -850,94 +794,72 @@ __device__ __forceinline__ void pk_tile(const PkArgs& a, const PkShared& sh, con
   }
   unsigned int unc_mask = 0u, unc_bit = 1u;  // deferred verdicts of this tile: bit p * K + j
   int pend_bin[K];  // image bin of the previous pose's verdict, -1 = not counted
-  int pend_inc[K];  // ATOM == 1: 0 / 1
 #pragma unroll
-  for (int j = 0; j < K; j++) pend_bin[j] = -1, pend_inc[j] = 0;
+  for (int j = 0; j < K; j++) pend_bin[j] = -1;
   unsigned int pend_off = 0;
   // :49 hist(image_bin, lidar_bin)++ for the previous pose's verdicts
   auto count_previous = [&]() {
 #pragma unroll
-    for (int j = 0; j < K; j++) {
-      if constexpr (ATOM == 0) {
-        if (pend_bin[j] >= 0) red_shared_inc(lb[j] + pend_off + 4u * static_cast<unsigned int>(pend_bin[j]));
-      } else {
-        red_shared_add(lb[j] + pend_off + 4u * static_cast<unsigned int>(pend_bin[j]), pend_inc[j]);
-      }
-    }
+    for (int j = 0; j < K; j++)
+      if (pend_bin[j] >= 0) red_shared_inc(lb[j] + pend_off + 4u * static_cast<unsigned int>(pend_bin[j]));
   };
   // the image-bin gathers of pose p's accepted verdicts, consumed by count_previous one pose later
-  auto gather = [&](int p, const bool (&acc)[K], const int (&pix)[K], const int (&wx)[K], const int (&wy)[K]) {
+  auto gather = [&](int p, const bool (&acc)[K], const int (&pix)[K]) {
     pend_off = 4u * static_cast<unsigned int>(p * a.nb);
 #pragma unroll
-    for (int j = 0; j < K; j++) {
-      if constexpr (TMA) {
-        const unsigned int dx = static_cast<unsigned int>(wx[j] - w.win_x0b), dy = static_cast<unsigned int>(wy[j] - w.win_y0b);
-        const bool inw = acc[j] & (dx < w.win_w) & (dy < w.win_h);
-        const bool out = acc[j] & !inw;
-        pend_bin[j] = gather_u8_window(inw, out, w.win_addr + dy * w.win_w + dx, B.bin_image + pix[j], ATOM == 0 ? -1 : 0);
-        if constexpr (ATOM != 0) pend_inc[j] = acc[j] ? 1 : 0;
-        w.n_window += inw ? 1u : 0u;
-        w.n_escaped += out ? 1u : 0u;
-      } else if constexpr (ATOM == 0) {
-        pend_bin[j] = ldg_u8_or_neg(acc[j], B.bin_image + pix[j]);
-      } else {
-        pend_bin[j] = ldg_u8_or_zero(acc[j], B.bin_image + pix[j]);
-        pend_inc[j] = acc[j] ? 1 : 0;
-      }
-    }
+    for (int j = 0; j < K; j++) pend_bin[j] = ldg_u8_or_neg(acc[j], B.bin_image + pix[j]);
   };
   // verdicts of points j, j + 1 from the packed classifier
-  auto record2 = [&](const LeanVerdict2& v, int j, bool (&acc)[K], int (&pix)[K], int (&wx)[K], int (&wy)[K]) {
+  auto record2 = [&](const LeanVerdict2& v, int j, bool (&acc)[K], int (&pix)[K]) {
 #pragma unroll
     for (int h = 0; h < 2; h++) {
       acc[j + h] = v.accept[h];
       if (v.uncertain[h]) unc_mask |= unc_bit << (j + h);
       pix[j + h] = v.idx[h];
-      if constexpr (TMA) wx[j + h] = v.ixb[h], wy[j + h] = v.iyb[h];
     }
   };
   // Equirectangular batches whose poses lie close together (sh.delta_on, set with the poses): pose 0 is the anchor, poses
   // 1..P-1 are first-order updates from it (classify_lean2_delta; bound and guards in lean_filter.cuh)
-  constexpr bool DELTA = DPOSE && PK_DELTA_POSES && PACKED && MODEL == CAM_EQUIRECTANGULAR && !TMA;
+  constexpr bool DELTA = DPOSE && PK_DELTA_POSES && PACKED && MODEL == CAM_EQUIRECTANGULAR;
   const bool delta_tile = DELTA && sh.delta_on;
   if (delta_tile) {
     if constexpr (DELTA) {
       LeanAnchor2 an[K / 2];
       {
         bool acc[K];
-        int pix[K], wx[K], wy[K];
+        int pix[K];
         const float4 r0 = sh.pose32[0][0], r1 = sh.pose32[0][1], r2 = sh.pose32[0][2];
         const float Pm[12] = {r0.x, r0.y, r0.z, r1.x, r1.y, r1.z, r2.x, r2.y, r2.z, r0.w, r1.w, r2.w};
 #pragma unroll
         for (int j = 0; j < K; j += 2)
-          record2(classify_lean2_anchor<MODEL>(a.fast, a.lean, a.width, Pm, X2[j / 2], Y2[j / 2], Z2[j / 2], D2[j / 2], an[j / 2]), j, acc, pix, wx, wy);
+          record2(classify_lean2_anchor<MODEL>(a.fast, a.lean, a.width, Pm, X2[j / 2], Y2[j / 2], Z2[j / 2], D2[j / 2], an[j / 2]), j, acc, pix);
         unc_bit <<= K;
-        gather(0, acc, pix, wx, wy);
+        gather(0, acc, pix);
       }
       for (int p = 1; p < n_poses; p++) {
         bool acc[K];
-        int pix[K], wx[K], wy[K];
+        int pix[K];
         const float4 q0 = sh.dpose[p][0], q1 = sh.dpose[p][1], q2 = sh.dpose[p][2], q3 = sh.dpose[p][3];
         const float Q[14] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, q3.x, q3.y};
 #pragma unroll
-        for (int j = 0; j < K; j += 2) record2(classify_lean2_delta<MODEL>(a.lean, a.width, Q, X2[j / 2], Y2[j / 2], Z2[j / 2], D2[j / 2], an[j / 2]), j, acc, pix, wx, wy);
+        for (int j = 0; j < K; j += 2) record2(classify_lean2_delta<MODEL>(a.lean, a.width, Q, X2[j / 2], Y2[j / 2], Z2[j / 2], D2[j / 2], an[j / 2]), j, acc, pix);
         unc_bit <<= K;
         count_previous();
-        gather(p, acc, pix, wx, wy);
+        gather(p, acc, pix);
       }
       count_previous();
     }
   } else {
     for (int p = 0; p <= n_poses; p++) {
       bool acc[K];
-      int pix[K], wx[K], wy[K];
+      int pix[K];
       if (p < n_poses) {
         const float4 r0 = sh.pose32[p][0], r1 = sh.pose32[p][1], r2 = sh.pose32[p][2];
         const float Pm[12] = {r0.x, r0.y, r0.z, r1.x, r1.y, r1.z, r2.x, r2.y, r2.z, r0.w, r1.w, r2.w};
         if constexpr (PACKED) {
 #pragma unroll
           for (int j = 0; j < K; j += 2)  // two points per instruction on the packed fp32 pipe (lean_filter2.cuh)
-            record2(classify_lean2<MODEL>(a.fast, a.lean, a.width, Pm, X2[j / 2], Y2[j / 2], Z2[j / 2], D2[j / 2]), j, acc, pix, wx, wy);
+            record2(classify_lean2<MODEL>(a.fast, a.lean, a.width, Pm, X2[j / 2], Y2[j / 2], Z2[j / 2], D2[j / 2]), j, acc, pix);
         } else {
 #pragma unroll
           for (int j = 0; j < K; j++) {
@@ -946,13 +868,12 @@ __device__ __forceinline__ void pk_tile(const PkArgs& a, const PkShared& sh, con
             const bool unc = PARTIAL ? (v.uncertain & valid0) : v.uncertain;
             if (unc) unc_mask |= unc_bit << j;
             pix[j] = v.idx;
-            if constexpr (TMA) wx[j] = v.ixb, wy[j] = v.iyb;
           }
         }
         unc_bit <<= K;
       }
       count_previous();
-      if (p < n_poses) gather(p, acc, pix, wx, wy);
+      if (p < n_poses) gather(p, acc, pix);
     }
   }
   // Deferred (point, pose) pairs of this tile -> the warp's queue for the exact path.  Doing this once per tile instead of inside the pose loop
@@ -1025,7 +946,7 @@ __device__ __forceinline__ void pk_load_tile(const float4* __restrict__ pts, uns
 }
 
 // points [tpos, end) of the cloud in single-row tiles, the next row in flight
-template <int MODEL, int ATOM, bool TMA>
+template <int MODEL>
 __device__ __forceinline__ void pk_rows(const PkArgs& a, const PkShared& sh, const PkBagRegs& B, int n_poses, PkWarp& w, unsigned int tpos, unsigned int end) {
   const int lane = w.lane;
   float4 q1[1], n1[1];
@@ -1033,30 +954,10 @@ __device__ __forceinline__ void pk_rows(const PkArgs& a, const PkShared& sh, con
   while (tpos < end) {
     const bool more = tpos + 32u < end;
     if (more) pk_load_tile<1>(B.points, tpos + 32u, end, lane, n1);
-    pk_tile<MODEL, 1, true, ATOM, TMA>(a, sh, B, n_poses, w, tpos, end, q1);
+    pk_tile<MODEL, 1, true>(a, sh, B, n_poses, w, tpos, end, q1);
     tpos += 32u;
     if (more) q1[0] = n1[0];
   }
-}
-
-// points [tpos, end) of the cloud: K-row tiles with the next tile's rows in flight, then single-row tiles for the rest;
-// qk holds the first K-row tile when `first_loaded`
-template <int MODEL, int K, int ATOM, bool TMA>
-__device__ __forceinline__ void pk_range(const PkArgs& a, const PkShared& sh, const PkBagRegs& B, int n_poses, PkWarp& w, unsigned int tpos, unsigned int end, float4 (&qk)[K], bool first_loaded) {
-  const int lane = w.lane;
-  if (!first_loaded && tpos + 32u * K <= end) pk_load_tile<K>(B.points, tpos, end, lane, qk);
-  while (tpos + 32u * K <= end) {
-    float4 nxt[K];
-    const bool more = tpos + 64u * K <= end;
-    if (more) pk_load_tile<K>(B.points, tpos + 32u * K, end, lane, nxt);
-    pk_tile<MODEL, K, false, ATOM, TMA>(a, sh, B, n_poses, w, tpos, end, qk);
-    tpos += 32u * K;
-    if (more) {
-#pragma unroll
-      for (int j = 0; j < K; j++) qk[j] = nxt[j];
-    }
-  }
-  pk_rows<MODEL, ATOM, TMA>(a, sh, B, n_poses, w, tpos, end);
 }
 
 // ---- tile ring: per warp, PK_RING shared-memory slots of one tile each, filled by cp.async -------------------------------
@@ -1108,14 +1009,14 @@ __device__ __forceinline__ void pk_stamp(const PkArgs& a, unsigned long long bat
 // DPOSE: this instance carries the equirectangular delta step (instantiated for equirectangular, K = 2 only; the host
 // picks it for Nelder-Mead solves and for pose lists with a chunk inside the gate, see pk_pick).  Its anchor state costs
 // registers in the whole kernel, so the plain instance stays for everything else.
-template <int MODEL, int K, int ATOM, bool TMA = false, bool DPOSE = false>
-__global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kernel(const __grid_constant__ PkArgs a) {
+template <int MODEL, int K, bool DPOSE = false>
+__global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __grid_constant__ PkArgs a) {
   extern __shared__ __align__(128) int smem_hist[];
   __shared__ PkShared sh;
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const bool solve_mode = a.solve != nullptr;
 
-  // block -> bag, warp -> fixed slice of the bag's cloud
+  // block -> bag, warp -> its interleaved tiles of the bag's cloud
   int bag = 0;
   while (bag + 1 < a.n_bags && static_cast<int>(blockIdx.x) >= a.bag[bag + 1].block_begin) bag++;
   const PkBag& Bc = a.bag[bag];
@@ -1125,13 +1026,6 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
   const unsigned int bag_n = Bc.n, bag_block_begin = static_cast<unsigned int>(Bc.block_begin), bag_block_count = static_cast<unsigned int>(Bc.block_count);
   const unsigned int warps_total = bag_block_count * PK_WARPS;
   const unsigned int warp_global = (blockIdx.x - bag_block_begin) * PK_WARPS + warp;
-  // points per warp: whole K-row tiles (a warp whose slice ends in single-row tiles runs them without instruction-level
-  // parallelism: at C2 that was 2 of its 3 tiles)
-  const unsigned int chunk = ((bag_n + warps_total - 1) / warps_total + (32u * K - 1u)) / (32u * K) * (32u * K);
-  const unsigned long long lo = static_cast<unsigned long long>(warp_global) * chunk;
-  const bool has_work = lo < bag_n;
-  const unsigned int end = has_work ? static_cast<unsigned int>(min(static_cast<unsigned long long>(bag_n), lo + chunk)) : 0u;
-  const unsigned int begin = static_cast<unsigned int>(has_work ? lo : 0ull);
 
   PkWarp w;
   w.lane = lane;
@@ -1142,11 +1036,10 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
   if (lane == 0) sh.q_cnt[warp] = 0, sh.deferred[warp][0] = sh.deferred[warp][1] = 0u;
   w.qn = 0;
   const unsigned int smem_base = static_cast<unsigned int>(__cvta_generic_to_shared(smem_hist));
-  // tile ring of this warp (interleaved split): this lane's rows of slot s at pk_ring_slot<K>(a, smem_base, s).  The pass's
+  // tile ring of this warp: this lane's rows of slot s at pk_ring_slot<K>(a, smem_base, s).  The pass's
   // bookkeeping {next tile, tiles left, tile step, slot} lives in sh.ring_state[warp] (every lane writes the same values and
   // reads them back).  While a tile is scored it waits there instead of in registers live across the pose loop.
-  constexpr bool RING = PK_TILE_RING && !TMA;
-  constexpr bool DELTA = DPOSE && PK_DELTA_POSES && PK_PACKED_FP32 && MODEL == CAM_EQUIRECTANGULAR && K % 2 == 0 && !TMA && PK_TILE_RING;  // as in pk_tile
+  constexpr bool DELTA = DPOSE && PK_DELTA_POSES && MODEL == CAM_EQUIRECTANGULAR && K % 2 == 0;  // as in pk_tile
   const unsigned int ring_state = static_cast<unsigned int>(__cvta_generic_to_shared(&sh.ring_state[warp]));
   const int n_items_per_batch = a.n_bags * (solve_mode ? PK_MAX_POSES : a.chunk);  // finalizer items of a full pose-list chunk
   const int fin_stride = max(1, static_cast<int>(gridDim.x) / (a.n_bags * PK_MAX_POSES));
@@ -1175,79 +1068,8 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
     sh.seq_base = *a.seq_counter;
     sh.trace_count = 0;
     sh.poses_scored = 0ull;
-    sh.bb_min_x = sh.bb_min_y = INT_MAX;
-    sh.bb_max_x = sh.bb_max_y = INT_MIN;
-    sh.box_w = sh.box_h = 0;
   }
   __syncthreads();
-  w.win_addr = 0, w.win_x0b = w.win_y0b = 0, w.win_w = w.win_h = 0, w.n_window = w.n_escaped = 0;
-  if constexpr (TMA) {
-    // ---- stage this block's window of the image-bin plane once for the whole solve (static split, Nelder-Mead mode) ----
-    // bounding box of the block's points at the first candidate (= the start pose), grown by a halo for the poses the solve
-    // will visit; pixels outside the window fall back to the global gather (counted in tma_stats[1])
-    const unsigned int win_base = smem_base + 4u * static_cast<unsigned int>(a.copies * PK_MAX_POSES * a.nb);  // 128-byte aligned (host)
-    if (solve_mode) {
-      int mnx = INT_MAX, mxx = INT_MIN, mny = INT_MAX, mxy = INT_MIN;
-      if (has_work) {
-        const float4 r0 = sh.pose32[0][0], r1 = sh.pose32[0][1], r2 = sh.pose32[0][2];
-        const float Pm[12] = {r0.x, r0.y, r0.z, r1.x, r1.y, r1.z, r2.x, r2.y, r2.z, r0.w, r1.w, r2.w};
-        const float tm = sh.pose32[0][3].x;
-        for (unsigned int i = begin + lane; i < end; i += 32u) {
-          const float4 q = __ldg(B.points + i);
-          const float dl = (5.25f * F32_U) * (fabsf(q.x) + fabsf(q.y) + fabsf(q.z) + tm);
-          const LeanVerdict v = classify_lean<MODEL>(a.fast, a.lean, a.width, Pm, q.x, q.y, q.z, dl);
-          if (v.accept) mnx = min(mnx, v.ixb), mxx = max(mxx, v.ixb), mny = min(mny, v.iyb), mxy = max(mxy, v.iyb);
-        }
-      }
-      mnx = __reduce_min_sync(0xffffffffu, mnx), mny = __reduce_min_sync(0xffffffffu, mny);
-      mxx = __reduce_max_sync(0xffffffffu, mxx), mxy = __reduce_max_sync(0xffffffffu, mxy);
-      if (lane == 0 && mnx <= mxx) {
-        atomicMin(&sh.bb_min_x, mnx), atomicMax(&sh.bb_max_x, mxx);
-        atomicMin(&sh.bb_min_y, mny), atomicMax(&sh.bb_max_y, mxy);
-      }
-      __syncthreads();
-      const unsigned int bar = static_cast<unsigned int>(__cvta_generic_to_shared(&sh.tma_bar));
-      if (t == 0 && sh.bb_min_x <= sh.bb_max_x) {
-        const int x0 = ((sh.bb_min_x - LEAN_MAGIC_BITS) - PK_TMA_HALO) & ~15;  // pixel coordinates; may be negative: TMA zero-fills
-        const int x1 = (sh.bb_max_x - LEAN_MAGIC_BITS) + PK_TMA_HALO;
-        const int y0 = (sh.bb_min_y - LEAN_MAGIC_BITS) - PK_TMA_HALO;
-        const int y1 = (sh.bb_max_y - LEAN_MAGIC_BITS) + PK_TMA_HALO;
-        const int nbx = (x1 - x0 + PK_TMA_BOX_W) / PK_TMA_BOX_W;
-        int rows = y1 - y0 + 1;
-        if (nbx * PK_TMA_BOX_W <= PK_TMA_BYTES) {
-          rows = min(rows, PK_TMA_BYTES / (nbx * PK_TMA_BOX_W));
-          sh.box_x0b = x0 + LEAN_MAGIC_BITS, sh.box_y0b = y0 + LEAN_MAGIC_BITS;
-          sh.box_w = nbx * PK_TMA_BOX_W, sh.box_h = rows;
-          asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar) : "memory");
-          asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(static_cast<unsigned int>(rows * nbx * PK_TMA_BOX_W)) : "memory");
-          const unsigned long long tmap = reinterpret_cast<unsigned long long>(&a.tmap[bag]);
-          for (int r = 0; r < rows; r++) {
-            for (int bx = 0; bx < nbx; bx++) {
-              const unsigned int dst = win_base + static_cast<unsigned int>((r * nbx + bx) * PK_TMA_BOX_W);
-              asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst), "l"(tmap),
-                           "r"(x0 + bx * PK_TMA_BOX_W), "r"(y0 + r), "r"(bar)
-                           : "memory");
-            }
-          }
-        }
-      }
-      __syncthreads();
-      if (sh.box_w > 0) {  // every thread waits for the bytes (phase 0); bounded, so that a refused descriptor cannot hang the GPU
-        unsigned int done = 0;
-        for (int spin = 0; spin < (1 << 22) && !done; spin++) {
-          asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(bar) : "memory");
-        }
-        if (!done) {
-          atomicExch(a.abort_flag, 1u);
-          if (a.error_host) *reinterpret_cast<volatile int*>(a.error_host) = 2;
-        }
-        w.win_addr = win_base, w.win_x0b = sh.box_x0b, w.win_y0b = sh.box_y0b;
-        w.win_w = static_cast<unsigned int>(sh.box_w), w.win_h = static_cast<unsigned int>(sh.box_h);
-      }
-    }
-  }
 
   for (unsigned long long batch = 0;; batch++) {
     const int n_poses = sh.n_poses;
@@ -1271,94 +1093,52 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
     // ---- (A) histograms of this block's share of the cloud ----------------------------------------------------------
     const int per_copy = n_poses * a.nb;
     w.hist_addr = smem_base + 4u * static_cast<unsigned int>((warp % a.copies) * per_copy);
-    if constexpr (TMA) {
-      // TMA variant: contiguous slice per warp (its image window must be compact)
-      float4 qk[K];
-      const bool preloaded = has_work && begin + 32u * K <= end;
-      if (preloaded) pk_load_tile<K>(B.points, begin, end, lane, qk);
-      if (fresh) {
-        for (int i = t; i < a.copies * per_copy; i += PK_THREADS) smem_hist[i] = 0;
-        __syncthreads();
-      }
-      if (time_block) a.block_times[4 * blockIdx.x + 1] = global_ns();
-      if (has_work) pk_range<MODEL, K, ATOM, TMA>(a, sh, B, n_poses, w, begin, end, qk, preloaded);
-    } else {
-      // Interleaved split: tile k (32 * K consecutive points of the tile-ordered cloud) goes to warp k mod W of the bag, so
-      // every warp -- and every block: its 24 warps take 24 neighbouring tiles per round -- samples the whole image instead of
-      // owning one region.  With contiguous slices the cost of a slice followed its region (deferred rechecks, histogram bin
-      // collisions, cache hit rates), so the slowest block finished well after the median one, and every Nelder-Mead batch
-      // waits for the slowest.  (Claiming tiles from an atomic counter was tried too: no better than the contiguous split
-      // at 256-point claims, and finer claims serialise on the counter.)
-      constexpr unsigned int TP = 32u * K;
-      if constexpr (RING) {
-        // The warp's full tiles stream through its shared-memory ring, PK_RING - 1 of them in flight behind the one being
-        // scored.  Serpentine sweep: odd passes walk the warp's tiles backwards, so every pass begins on the tiles that the
-        // previous one touched last (still in L2 when the cloud is larger than L2) -- same tiles, other order, same counts.
-        {
-          const unsigned int n_full = bag_n / TP;
-          const unsigned int nt = warp_global < n_full ? (n_full - 1u - warp_global) / warps_total + 1u : 0u;
-          const bool backward = (batch & 1ull) != 0ull;
-          const unsigned int step = backward ? 0u - warps_total : warps_total;  // tiles between consecutive steps (mod 2^32)
-          const unsigned int tile0 = backward ? warp_global + (nt - 1u) * warps_total : warp_global;
+    // Interleaved split: tile k (32 * K consecutive points of the tile-ordered cloud) goes to warp k mod W of the bag, so
+    // every warp -- and every block: its 24 warps take 24 neighbouring tiles per round -- samples the whole image instead of
+    // owning one region.  With contiguous slices the cost of a slice followed its region (deferred rechecks, histogram bin
+    // collisions, cache hit rates), so the slowest block finished well after the median one, and every Nelder-Mead batch
+    // waits for the slowest.  (Claiming tiles from an atomic counter was tried too: no better than the contiguous split
+    // at 256-point claims, and finer claims serialise on the counter.)
+    constexpr unsigned int TP = 32u * K;
+    // The warp's full tiles stream through its shared-memory ring, PK_RING - 1 of them in flight behind the one being
+    // scored.  Serpentine sweep: odd passes walk the warp's tiles backwards, so every pass begins on the tiles that the
+    // previous one touched last (still in L2 when the cloud is larger than L2) -- same tiles, other order, same counts.
+    {
+      const unsigned int n_full = bag_n / TP;
+      const unsigned int nt = warp_global < n_full ? (n_full - 1u - warp_global) / warps_total + 1u : 0u;
+      const bool backward = (batch & 1ull) != 0ull;
+      const unsigned int step = backward ? 0u - warps_total : warps_total;  // tiles between consecutive steps (mod 2^32)
+      const unsigned int tile0 = backward ? warp_global + (nt - 1u) * warps_total : warp_global;
 #pragma unroll
-          for (int s = 0; s + 1 < PK_RING; s++)
-            pk_ring_fill<K>(pk_ring_slot<K>(a, smem_base, s), B.points + static_cast<size_t>(tile0 + s * step) * TP + lane, static_cast<unsigned int>(s) < nt);
-          sts_v4(ring_state, make_uint4(tile0, nt, step, 0u));
-        }
-        if (fresh) {
-          for (int i = t; i < a.copies * per_copy; i += PK_THREADS) smem_hist[i] = 0;
-          __syncthreads();
-        }
-        if (time_block) a.block_times[4 * blockIdx.x + 1] = global_ns();
-        for (;;) {
-          const uint4 rs = lds_v4(ring_state);  // {tile, tiles left, step, slot}
-          if (rs.y == 0u) break;
-          // this lane's copies of the tile landed (the later groups may still be in flight)
-          asm volatile("cp.async.wait_group %0;" ::"n"(PK_RING - 2) : "memory");
-          const unsigned int row0 = pk_ring_slot<K>(a, smem_base, rs.w);
-          float4 q[K];
-#pragma unroll
-          for (int j = 0; j < K; j++) {
-            asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(q[j].x), "=f"(q[j].y), "=f"(q[j].z), "=f"(q[j].w) : "r"(row0 + 512u * j) : "memory");
-          }
-          // refill the slot read at the step before (its rows went through the pose loop) with the tile PK_RING - 1 steps ahead
-          const unsigned int refill = rs.w == 0u ? PK_RING - 1u : rs.w - 1u;
-          pk_ring_fill<K>(pk_ring_slot<K>(a, smem_base, refill), B.points + static_cast<size_t>(rs.x + (PK_RING - 1) * rs.z) * TP + lane, rs.y > PK_RING - 1u);
-          sts_v4(ring_state, make_uint4(rs.x + rs.z, rs.y - 1u, rs.z, rs.w + 1u == PK_RING ? 0u : rs.w + 1u));
-          pk_tile<MODEL, K, false, ATOM, TMA, DPOSE>(a, sh, B, n_poses, w, rs.x * TP, bag_n, q);
-        }
-        // the cloud's ragged last tile (fewer than 32 * K points, register loads) belongs to the warp whose tile sequence reaches it
-        const unsigned int n_full = bag_n / TP;
-        if (n_full * TP < bag_n && n_full % warps_total == warp_global) pk_rows<MODEL, ATOM, TMA>(a, sh, B, n_poses, w, n_full * TP, bag_n);
-      } else {
-        // PK_TILE_RING=0 (A/B): the next tile's rows are in flight in registers while the current one is swept over the
-        // poses; every pass walks forwards
-        unsigned int tile = warp_global;
-        float4 qk[K];
-        bool full = static_cast<unsigned long long>(tile) * TP + TP <= bag_n;
-        if (full) pk_load_tile<K>(B.points, tile * TP, bag_n, lane, qk);
-        if (fresh) {
-          for (int i = t; i < a.copies * per_copy; i += PK_THREADS) smem_hist[i] = 0;
-          __syncthreads();
-        }
-        if (time_block) a.block_times[4 * blockIdx.x + 1] = global_ns();
-        while (full) {
-          const unsigned int ntile = tile + warps_total;
-          const bool nfull = static_cast<unsigned long long>(ntile) * TP + TP <= bag_n;
-          float4 nxt[K];
-          if (nfull) pk_load_tile<K>(B.points, ntile * TP, bag_n, lane, nxt);
-          pk_tile<MODEL, K, false, ATOM, TMA>(a, sh, B, n_poses, w, tile * TP, bag_n, qk);
-          tile = ntile;
-          full = nfull;
-          if (nfull) {
-#pragma unroll
-            for (int j = 0; j < K; j++) qk[j] = nxt[j];
-          }
-        }
-        // the cloud's ragged last tile (fewer than 32 * K points) belongs to whichever warp's sequence reaches it
-        if (static_cast<unsigned long long>(tile) * TP < bag_n) pk_range<MODEL, K, ATOM, TMA>(a, sh, B, n_poses, w, tile * TP, bag_n, qk, false);
-      }
+      for (int s = 0; s + 1 < PK_RING; s++)
+        pk_ring_fill<K>(pk_ring_slot<K>(a, smem_base, s), B.points + static_cast<size_t>(tile0 + s * step) * TP + lane, static_cast<unsigned int>(s) < nt);
+      sts_v4(ring_state, make_uint4(tile0, nt, step, 0u));
     }
+    if (fresh) {
+      for (int i = t; i < a.copies * per_copy; i += PK_THREADS) smem_hist[i] = 0;
+      __syncthreads();
+    }
+    if (time_block) a.block_times[4 * blockIdx.x + 1] = global_ns();
+    for (;;) {
+      const uint4 rs = lds_v4(ring_state);  // {tile, tiles left, step, slot}
+      if (rs.y == 0u) break;
+      // this lane's copies of the tile landed (the later groups may still be in flight)
+      asm volatile("cp.async.wait_group %0;" ::"n"(PK_RING - 2) : "memory");
+      const unsigned int row0 = pk_ring_slot<K>(a, smem_base, rs.w);
+      float4 q[K];
+#pragma unroll
+      for (int j = 0; j < K; j++) {
+        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(q[j].x), "=f"(q[j].y), "=f"(q[j].z), "=f"(q[j].w) : "r"(row0 + 512u * j) : "memory");
+      }
+      // refill the slot read at the step before (its rows went through the pose loop) with the tile PK_RING - 1 steps ahead
+      const unsigned int refill = rs.w == 0u ? PK_RING - 1u : rs.w - 1u;
+      pk_ring_fill<K>(pk_ring_slot<K>(a, smem_base, refill), B.points + static_cast<size_t>(rs.x + (PK_RING - 1) * rs.z) * TP + lane, rs.y > PK_RING - 1u);
+      sts_v4(ring_state, make_uint4(rs.x + rs.z, rs.y - 1u, rs.z, rs.w + 1u == PK_RING ? 0u : rs.w + 1u));
+      pk_tile<MODEL, K, false, DPOSE>(a, sh, B, n_poses, w, rs.x * TP, bag_n, q);
+    }
+    // the cloud's ragged last tile (fewer than 32 * K points, register loads) belongs to the warp whose tile sequence reaches it
+    const unsigned int n_full = bag_n / TP;
+    if (n_full * TP < bag_n && n_full % warps_total == warp_global) pk_rows<MODEL>(a, sh, B, n_poses, w, n_full * TP, bag_n);
     if (w.qn > 0) {
       pk_drain32<MODEL>(a, sh, B, w, 0, w.qn);
       w.qn = 0;
@@ -1448,7 +1228,7 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
     // batch - 1 (finished by every block before it arrived here) and is next merged in batch + 2, which no block reaches
     // before every block arrived for batch + 1, i.e. after this block's zeroing (ordered by the arrival fence).
     if (!pk_wait_arrivals(a, a.arrive + buf * PK_MAX_BAGS, static_cast<unsigned int>(batch / 3ull + 1ull))) return;
-    if (!PK_DIAG_STAMPS && blockIdx.x == 0 && t == 0) pk_stamp(a, batch, 3);
+    if (blockIdx.x == 0 && t == 0) pk_stamp(a, batch, 3);
     {
       const int nz = a.n_bags * PK_MAX_POSES * a.nb;
       int* z = a.ghist + static_cast<size_t>((buf + 2) % 3) * nz;
@@ -1466,12 +1246,7 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
       const int round_items = min(PK_WARPS, (a.copies * PK_MAX_POSES * a.nb * 4) / pk_fin_item_bytes(a.nb, a.bins));
       for (int first = 0; first < n_items; first += round_items) {
         const int count = min(round_items, n_items - first);
-        unsigned long long* diag = nullptr;
-        if (PK_DIAG_STAMPS && blockIdx.x == 0 && first == 0 && a.stamps && batch < static_cast<unsigned long long>(a.stamps_cap)) {
-          diag = a.stamps + batch * PK_STAMP_SLOTS + 5;
-          if (t == 0) pk_stamp(a, batch, 3);
-        }
-        pk_block_nid_items(gbuf, mbuf, first, count, n_poses, a.nb, a.bins, smem_hist, sh.fin_out, diag);
+        pk_block_nid_items(gbuf, mbuf, first, count, n_poses, a.nb, a.bins, smem_hist, sh.fin_out);
         if (t < count) {
           const int item = first + t, ib = item / n_poses, ip = item - ib * n_poses;
           const int word = (a.rank * a.n_bags + ib) * PK_MAX_POSES + ip;
@@ -1519,7 +1294,7 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
       sh.parts[src * PK_MAX_POSES + p] = __longlong_as_double(static_cast<long long>((wh << 32) | (wl & 0xffffffffull)));
     }
     if (__syncthreads_or(timed_out ? 1 : 0)) return;
-    if (!PK_DIAG_STAMPS && blockIdx.x == 0 && t == 0) pk_stamp(a, batch, 5);
+    if (blockIdx.x == 0 && t == 0) pk_stamp(a, batch, 5);
     if (t < n_poses) {
       double total = 0.0;
       for (int s = 0; s < a.world * a.n_bags; s++) total += sh.parts[s * PK_MAX_POSES + t];  // (rank, bag) order: identical everywhere
@@ -1566,15 +1341,6 @@ __global__ void __launch_bounds__(PK_THREADS, PK_MIN_BLOCKS) nid_persistent_kern
     atomicAdd(a.delta_stats + 2, static_cast<unsigned long long>(sh.deferred[warp][0]));
     atomicAdd(a.delta_stats + 3, static_cast<unsigned long long>(sh.deferred[warp][1]));
   }
-  if constexpr (TMA) {
-    if (a.tma_stats) {
-      const unsigned int nw = __reduce_add_sync(0xffffffffu, w.n_window), ne = __reduce_add_sync(0xffffffffu, w.n_escaped);
-      if (lane == 0) {
-        atomicAdd(a.tma_stats + 0, static_cast<unsigned long long>(nw));
-        atomicAdd(a.tma_stats + 1, static_cast<unsigned long long>(ne));
-      }
-    }
-  }
   // ---- results (block 0) ----
   if (blockIdx.x == 0) {
     if (solve_mode) {
@@ -1610,7 +1376,7 @@ __global__ void __launch_bounds__(NID_THREADS) nid_lean_verify_kernel(const __gr
     for (int p = 1; p < a.n_poses; p++) lean_delta_pose(a.pose[p], a.pose[0], Q[p]);
   }
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
-  // points in pairs (2k, 2k + 1), as the hot loop classifies them when the packed classifier is compiled in
+  // points in pairs (2k, 2k + 1), as the hot loop classifies them with the packed classifier
   for (long long k = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; 2 * k < a.n; k += stride) {
     const long long i0 = 2 * k, i1 = min(2 * k + 1, static_cast<long long>(a.n) - 1);
     const int n_here = 2 * k + 1 < a.n ? 2 : 1;
@@ -1627,7 +1393,7 @@ __global__ void __launch_bounds__(NID_THREADS) nid_lean_verify_kernel(const __gr
           v2[h].accept = w.accept[h], v2[h].uncertain = w.uncertain[h], v2[h].idx = w.idx[h];
           v2[h].up = w.up[h], v2[h].vp = w.vp[h], v2[h].hx = w.hx[h], v2[h].hy = w.hy[h];
         }
-      } else if constexpr (PK_PACKED_FP32 && LeanPacked<MODEL>::value) {
+      } else if constexpr (LeanPacked<MODEL>::value) {
         const LeanVerdict2 w = classify_lean2<MODEL>(a.fast, lc, a.width, a.pose32[p], f2_pack(q2[0].x, q2[1].x), f2_pack(q2[0].y, q2[1].y),
                                                      f2_pack(q2[0].z, q2[1].z), f2_pack(delta[0], delta[1]));
         for (int h = 0; h < 2; h++) {

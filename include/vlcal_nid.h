@@ -174,13 +174,11 @@ int vlcal_nid_debug_solve_stamps(vlcal_nid_ctx* ctx, int capacity, uint64_t* sta
 /* with the stamps armed, every block of the persistent solve also records {enters the batch, histogram copies zeroed, main
  * loop done, arrived} for one batch (the 9th): capacity_blocks x 4 words out, *n_blocks = blocks of that launch */
 int vlcal_nid_debug_block_times(vlcal_nid_ctx* ctx, int capacity_blocks, uint64_t* times_out, int* n_blocks);
-/* TMA variant of the persistent solve (environment VLCAL_PK_TMA=1; A/B measurement, off by default): image-bin gathers of
- * the last solve served from the shared-memory window each block staged with cp.async.bulk.tensor, and gathers that fell
- * outside it and went to global memory */
-int vlcal_nid_debug_tma_stats(vlcal_nid_ctx* ctx, uint64_t stats[2]);
-/* kernel selection for A/B measurements: 0 = default (fp32 filter + exact fp64 recheck; 2 or 4 points per lane and
- * tile, chosen from the camera model and the cloud size), 1 = exact fp64 only, 2 = filter forced to 2 points,
- * 3 = filter forced to 4 points, 4 = round-1 kernels (one launch per batch; the persistent kernel is not used) */
+/* kernel selection for A/B measurements: 0 = default (fp32 filter + exact fp64 recheck; the persistent kernel at 2 points
+ * per lane and tile, the round-1 kernels, where they run, at 2 or 4 chosen from the camera model and the cloud size),
+ * 1 = exact fp64 only, 2 = filter forced to 2 points, 3 = filter forced to 4 points (in the persistent kernel for
+ * plumb_bob, omnidir and rational_polynomial only; the other models keep 2), 4 = round-1 kernels (one launch per batch;
+ * the persistent kernel is not used) */
 int vlcal_nid_set_kernel_variant(vlcal_nid_ctx* ctx, int variant);
 
 /* measurement hook: one launch (n_poses <= 8) with %globaltimer stamps; out_us = {main loop done, merged, ticket, finalize done,

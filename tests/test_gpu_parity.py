@@ -589,44 +589,6 @@ def test_fused_peer_exchange_matches_nccl_and_single_gpu(gpu):
     assert "POSE_SHARD_CHECK world=2" in out.stdout and "identical=True" in out.stdout.split("POSE_SHARD_CHECK")[1]
 
 
-def test_tma_window_variant_walks_the_same_trajectory(gpu):
-    """VLCAL_PK_TMA=1: every block stages its window of the image-bin plane in shared memory with cp.async.bulk.tensor once
-    per solve and gathers from it (global-memory fallback outside the window).  Same bits as the default kernel and as the
-    round-1 host loop; most gathers must be served by the window."""
-    import subprocess
-    import sys
-
-    code = (
-        "import numpy as np, sys\n"
-        "sys.path.insert(0, 'tests')\n"
-        "import direct_visual_lidar_calibration_b200 as V\n"
-        "from direct_visual_lidar_calibration_b200 import calibration as VC, synthetic as S\n"
-        "bag = S.make_bag('pinhole_1920x1080', 'os1_64', 200000, config_index=1)\n"
-        "T0 = S.perturb(bag['T_gt'], (0.4, -0.3, 0.3), (0.01, -0.01, 0.02))\n"
-        "cam = V.create_camera(bag['camera_model'], bag['intrinsics'], bag['distortion'])\n"
-        "data = V.VisualLiDARData(bag['image'], bag['points'], bag['intensities'])\n"
-        "idx = V.ViewCulling(cam, (1920, 1080)).cull_indices(data.points, T0)\n"
-        "cost = V.CostCalculatorNID(cam, V.VisualLiDARData(bag['image'], data.points[idx], data.intensities[idx]))\n"
-        "cost.set_kernel_variant(2)\n"  # 2 points per lane: the shape the TMA variant is instantiated for
-        "cost.reorder_for_pose(T0)\n"
-        "p = V.VisualCameraCalibrationParams(); p.max_inner_iterations = 60\n"
-        "out = {}\n"
-        "for mode in (1, 3):\n"
-        "    V.set_solver_mode(mode)\n"
-        "    out[mode] = VC.estimate_pose_on_costs([cost], T0, p)\n"
-        "w, e = cost.tma_stats()\n"
-        "same = np.array_equal(out[1][0], out[3][0]) and out[1][1]['y'] == out[3][1]['y'] and out[1][1]['num_evaluations'] == out[3][1]['num_evaluations']\n"
-        "print('TMA_CHECK', same, w, e)\n"
-    )
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600, cwd=root, env=dict(os.environ, VLCAL_PK_TMA="1"))
-    assert out.returncode == 0, out.stdout[-2000:] + out.stderr[-2000:]
-    line = [ln for ln in out.stdout.splitlines() if ln.startswith("TMA_CHECK")][0].split()
-    assert line[1] == "True", out.stdout
-    window, escaped = int(line[2]), int(line[3])
-    assert window > 0 and window + escaped > 0, (window, escaped)
-
-
 def test_persistent_exchange_two_ranks_on_one_gpu(gpu):
     """The in-kernel score exchange of the persistent solve (tagged words in cudaIpc-shared mailboxes, summed in (rank, bag)
     order by every block of every rank) with TWO processes on ONE GPU -- so that the single-GPU test box covers it: one

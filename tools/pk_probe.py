@@ -74,8 +74,7 @@ def main():
             ref = (T, r)
         else:
             same = bool(np.array_equal(T, ref[0]) and r["y"] == ref[1]["y"] and r["num_evaluations"] == ref[1]["num_evaluations"])
-        tma = cost.tma_stats() if os.environ.get("VLCAL_PK_TMA") == "1" and mode == 3 else None
-        line = dict(base, what="solve", mode=mode, tma_window_vs_escaped=tma, ms_per_solve=1e3 * dt, evals=r["num_evaluations"], evals_per_s=r["num_evaluations"] / dt, batches=r["num_batches"],
+        line = dict(base, what="solve", mode=mode, ms_per_solve=1e3 * dt, evals=r["num_evaluations"], evals_per_s=r["num_evaluations"] / dt, batches=r["num_batches"],
                     us_per_batch=1e6 * dt / max(1, r["num_batches"]), computed=r["num_evaluations_computed"], gpp_per_s=n_culled * r["num_evaluations_computed"] / dt * 1e-9,
                     kernel_ms_per_solve=prof["kernel_ms_total"] / args.reps, passes=prof["passes"] / args.reps, launches=prof["kernel_launches"] / args.reps, y=r["y"], same_as_first_mode=same)
         print(json.dumps(line), flush=True)
