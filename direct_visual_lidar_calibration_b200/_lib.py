@@ -115,6 +115,14 @@ class ScanDesc(C.Structure):
     ]
 
 
+class SearchSet(C.Structure):
+    """vlcal_search_set: pose i = (ib * n_left + il) * n_offset + io is [R | R (center[ib] + offset[io])], R = left[il] base[ib]."""
+    _fields_ = [
+        ("left", C.POINTER(C.c_double)), ("base", C.POINTER(C.c_double)), ("center", C.POINTER(C.c_double)), ("offset", C.POINTER(C.c_double)),
+        ("indices", C.POINTER(C.c_int32)), ("n_left", C.c_int32), ("n_base", C.c_int32), ("n_offset", C.c_int32), ("n_poses", C.c_int64),
+    ]
+
+
 SE3_OBJECTIVE = C.CFUNCTYPE(C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_void_p)
 NM_BATCH_FN = C.CFUNCTYPE(None, C.POINTER(C.c_double), C.c_int, C.c_int, C.POINTER(C.c_double), C.c_void_p)
 NM_OBSERVE_FN = C.CFUNCTYPE(None, C.POINTER(C.c_double), C.c_int, C.c_double, C.c_void_p)
@@ -148,6 +156,14 @@ def load_library():
     L.vlcal_nid_evaluate_async.argtypes = [vp, dp, C.c_int]
     L.vlcal_nid_wait.argtypes = [vp, dp, vp]
     L.vlcal_nid_score_poses.argtypes = [C.POINTER(vp), C.c_int, dp, C.c_int, dp]
+    L.vlcal_nid_sweep_poses.argtypes = [C.POINTER(vp), C.c_int, dp, C.c_int64, dp, vp]
+    L.vlcal_nid_debug_sweep_kernel.argtypes = [C.POINTER(vp), C.c_int, dp, C.c_int64, dp, vp]
+    L.vlcal_nid_sweep_search_set.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(SearchSet), dp]
+    L.vlcal_nid_sweep_search_set_inliers.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(SearchSet), dp, C.POINTER(C.c_int64)]
+    L.vlcal_search_set_poses.argtypes = [C.c_int, C.POINTER(SearchSet), dp]
+    L.vlcal_nid_sweep_max_points.restype = C.c_int64
+    L.vlcal_nid_sweep_launch_shape.argtypes = [vp, ip, ip]
+    L.vlcal_nid_sweep_last_kernel_ms.restype = C.c_double
     L.vlcal_nid_set_poses_per_pass.argtypes = [vp, C.c_int]
     L.vlcal_nid_get_profile_passes.argtypes = [vp, C.POINTER(C.c_int64)]
     L.vlcal_nid_get_profile_delta.argtypes = [vp, C.POINTER(C.c_int64)]

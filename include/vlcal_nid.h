@@ -128,6 +128,51 @@ int vlcal_nid_wait(vlcal_nid_ctx* ctx, double* nid_out, int32_t* hist_out);
  * vlcal_nid_evaluate returns for that pose, bit for bit. */
 int vlcal_nid_score_poses(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_camera_lidar, int n_poses, double* nid_out);
 
+/* ---- pose sweep: very long pose lists on small clouds (the global initial-guess search) -----------------------------
+ * Same scores as vlcal_nid_score_poses -- nid_out[p] = sum over the contexts, in the order given, of
+ * CostCalculatorNID::calculate(T_p), bit for bit -- computed pose-parallel: one thread block owns a few poses from the
+ * first point to the finished NID, so 10^5-10^6 poses on 10^4-10^5 points fill the GPU, where the persistent kernel's
+ * pose-list mode (8 poses per pass, one block per 768 points) leaves most of it idle.  When the contexts hold more than
+ * vlcal_nid_sweep_max_points() points together the list is handed to that kernel instead (same results).
+ * Contexts: mode A, float4 clouds, bins <= 32, one camera / image size / bins / device, at most 8 of them; anything else
+ * is VLCAL_ERR_UNSUPPORTED.  hist_out: optional P x bins x bins int32 joint histograms of ctxs[0], laid out as in
+ * vlcal_nid_evaluate.  Synchronous. */
+int vlcal_nid_sweep_poses(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_camera_lidar, int64_t n_poses, double* nid_out, int32_t* hist_out);
+
+/* A pose list described by small tables instead of P matrices; the poses are generated on the device.  Pose i, with
+ * i = (ib * n_left + il) * n_offset + io:
+ *     R = left[il] * base[ib],   t = R * (center[ib] + offset[io]),   T_camera_lidar = [R | t]
+ * so with center = -(camera position in the LiDAR frame) the offsets move the camera position and leave the rotation
+ * alone.  Every product and sum is one IEEE round-to-nearest operation, row by row, ((a0*b0 + a1*b1) + a2*b2): a host that
+ * does the same operations gets the same bits.  indices: optional n_poses flat indices i (a subset, in any order); NULL
+ * means all n_base * n_left * n_offset poses in order, and n_poses must be that product. */
+typedef struct vlcal_search_set {
+  const double* left;   /* n_left x 9, row-major 3x3 */
+  const double* base;   /* n_base x 9 */
+  const double* center; /* n_base x 3 */
+  const double* offset; /* n_offset x 3 */
+  const int32_t* indices;
+  int32_t n_left, n_base, n_offset;
+  int64_t n_poses;
+} vlcal_search_set;
+
+/* vlcal_nid_sweep_poses for the poses of a search set (no upload of the matrices) */
+int vlcal_nid_sweep_search_set(vlcal_nid_ctx* const* ctxs, int n_ctxs, const vlcal_search_set* set, double* nid_out);
+/* the same, and per pose the number of points the reference counts (hist_image.sum(), cost_calculator_nid.cpp:54) summed
+ * over the contexts: a search uses it to set aside poses that see next to nothing, whose NID is meaninglessly low */
+int vlcal_nid_sweep_search_set_inliers(vlcal_nid_ctx* const* ctxs, int n_ctxs, const vlcal_search_set* set, double* nid_out, int64_t* inliers_out);
+/* the poses of a search set as the device generates them: n_poses x 16 doubles, column-major (device -1: the current one) */
+int vlcal_search_set_poses(int device, const vlcal_search_set* set, double* T_camera_lidar_out);
+/* cloud size (points of all contexts together) up to which the sweep kernel runs */
+int64_t vlcal_nid_sweep_max_points(void);
+/* launch geometry of the sweep kernel for this context's camera model: blocks that are resident at once on its device,
+ * and the poses one block scores together */
+int vlcal_nid_sweep_launch_shape(const vlcal_nid_ctx* ctx, int* blocks, int* poses_per_block);
+/* measurement hooks: the sweep kernel whatever the cloud size (the crossover measurement), and the kernel time of the
+ * calling thread's last sweep in milliseconds (CUDA events around the kernel; 0 when the persistent kernel ran instead) */
+int vlcal_nid_debug_sweep_kernel(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_camera_lidar, int64_t n_poses, double* nid_out, int32_t* hist_out);
+double vlcal_nid_sweep_last_kernel_ms(void);
+
 /* mode B evaluation with the reference's parameterisation: T_params = P x 7 doubles [qx qy qz qw tx ty tz]
  * (Sophus::SE3d storage, include/vlcal/costs/nid_cost.hpp:38).  ok_out[p] = 0 where the reference functor returns
  * false (non-finite NID, :98-102).  hist_out: optional P x bins x bins doubles (un-normalised). */
