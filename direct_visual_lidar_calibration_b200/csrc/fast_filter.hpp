@@ -177,16 +177,27 @@ inline LeanCam make_lean_cam(const CameraParams& cam, const FastCam& f, int widt
     c.eq_sv = static_cast<float>(2.0 * cam.intr[1]);
     c.cxh = static_cast<float>(0.5 * cam.intr[0] - 0.5);
     c.cyh = static_cast<float>(0.5 * cam.intr[1] - 0.5);
-    // u' = fma(lon_turns, W, W/2 - 0.5): the angle's error times W, one rounding of the result (|u'| <= W + 1) and the
-    // rounding of the constant (<= u W / 2); W itself is exact.  (project_fast charges 4u (W + Wd + 1) for its three-step
-    // form; the single FMA needs 2u (W + 1), which halves E and the deferral rate of this model.)
+    // u' = fma(lon_turns, W~, cxh~) (W~ = eq_su, cxh~ = cxh: the float copies of W and W/2 - 0.5) against the exact
+    // W L + W/2 - 0.5 (L: the longitude in turns).  With L~ the fp32 angle (|L~| <= 1/2: lean_atan2_turns returns at most
+    // 0.5 in magnitude) and z = L~ W~ + cxh~ the unrounded FMA,
+    //   u' - (W L + W/2 - 0.5) = (fl(z) - z) + L~ (W~ - W) + (cxh~ - (W/2 - 0.5)) + W (L~ - L),
+    // |fl(z) - z| <= u |z| <= u (W~ / 2 + |cxh~|) (one rounding to nearest; 1e-9 px covers an underflow).  The last term is
+    // the angle's error times W: LEAN_ATAN_ERR_TURNS here, the input-error term through sfx in the kernel.  Likewise v' =
+    // fma(lat_turns, 2H~, cyh~) with |lat~| <= 1/4 (atan2(y, r_xz) with r_xz >= 0 never takes the b < 0 fold).  For
+    // W = 3840 this is u (W - 1/2) + 0 + 0, half an ulp of the result at most.  (project_fast charges 4u (W + Wd + 1) for
+    // its three-step form.)
     (void)Wd, (void)Hd;
-    const double cu = SAFETY * (W * LEAN_ATAN_ERR_TURNS + 2.0 * U * (W + 1.0));
-    const double cv = SAFETY * (2.0 * H * LEAN_ATAN_ERR_TURNS + 2.0 * U * (H + 1.0));
+    const double Wf = c.eq_su, Sf = c.eq_sv, cxf = c.cxh, cyf = c.cyh;
+    const double ru = U * (0.5 * Wf + std::fabs(cxf)) + 0.5 * std::fabs(Wf - W) + std::fabs(cxf - (0.5 * W - 0.5)) + 1e-9;
+    const double rv = U * (0.25 * Sf + std::fabs(cyf)) + 0.25 * std::fabs(Sf - 2.0 * H) + std::fabs(cyf - (0.5 * H - 0.5)) + 1e-9;
+    const double cu = SAFETY * (W * LEAN_ATAN_ERR_TURNS + ru);
+    const double cv = SAFETY * (2.0 * H * LEAN_ATAN_ERR_TURNS + rv);
     c.hx0 = dn(0.5 - cu);
     c.hy0 = dn(0.5 - cv);
     if (!(c.hx0 > 0.0f) || !(c.hy0 > 0.0f)) return c;
-    // delta step (lean_filter.cuh, above classify_lean_delta): terms 2-4 of its bound
+    // delta step (lean_filter.cuh, above classify_lean_delta): terms 2-4 of its bound.  The rounding of up0 + s is at most
+    // u |up0 + s| with |up0| <= (W~ / 2 + |cxh~|)(1 + u) (as above) and |s| <= W / 32pi < 0.01 W; 0.02 W + 1 absorbs both
+    // excesses (likewise v with 2H~ / 4 + |cyh~| and 2H / 32pi).
     const double su = W, sv = 2.0 * H;
     c.eq_gu = static_cast<float>(su / (2.0 * M_PI));
     c.eq_gv = static_cast<float>(sv / (2.0 * M_PI));
@@ -194,8 +205,8 @@ inline LeanCam make_lean_cam(const CameraParams& cam, const FastCam& f, int widt
     c.eq_kv = up(SAFETY * sv / (4.0 * M_PI) * 1.2072 * 1.15);
     c.eq_lu = up(SAFETY * su / (2.0 * M_PI) / 8.07 * (1.0 + 1e-5));
     c.eq_lv = up(SAFETY * sv / (2.0 * M_PI) / 8.07 * (1.0 + 1e-5));
-    c.eq_cu = up(SAFETY * (64.0 * U * su / (32.0 * M_PI) + 2.0 * U * (1.03 * W + 1.0)) + 1e-6);
-    c.eq_cv = up(SAFETY * (64.0 * U * sv / (32.0 * M_PI) + 2.0 * U * (1.03 * H + 1.0)) + 1e-6);
+    c.eq_cu = up(SAFETY * (64.0 * U * su / (32.0 * M_PI) + U * (0.5 * Wf + std::fabs(cxf) + 0.02 * su + 1.0)) + 1e-6);
+    c.eq_cv = up(SAFETY * (64.0 * U * sv / (32.0 * M_PI) + U * (0.25 * Sf + std::fabs(cyf) + 0.02 * sv + 1.0)) + 1e-6);
     c.eq_hxd = dn(static_cast<double>(c.hx0) - static_cast<double>(c.eq_cu));
     c.eq_nsx15 = dn(1.5 * static_cast<double>(c.nsfx));
   }

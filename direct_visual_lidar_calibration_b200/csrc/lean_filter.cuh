@@ -56,23 +56,52 @@ struct LeanCam {
 };
 
 // atan2(a, b) / (2 pi) in turns, (-0.5, 0.5]: octant reduction + odd minimax polynomial of degree 13 on [0, 1] (fitted for
-// this file, tools/fit_atan_turns.py; fp32 Horner error <= 5.3e-8 turns) -- 20 instructions and one MUFU.RCP against ~40
-// for atan2f, whose special cases (infinities, signed zeros, denormals) the filter does not need: every degenerate input
-// comes out NaN or lands on a pixel edge, i.e. "uncertain".  Absolute error <= 1.1e-7 turns (polynomial 5.3e-8, quotient
-// rounding 1.4e-8, octant folds 4.5e-8); LEAN_ATAN_ERR_TURNS is what the error bound charges for it.
-constexpr double LEAN_ATAN_ERR_TURNS = 2.5e-7;
+// this file, tools/fit_atan_turns.py) -- 20 instructions and one MUFU.RCP against ~40 for atan2f, whose special cases
+// (infinities, signed zeros, denormals) the filter does not need: every degenerate input comes out NaN or lands on a pixel
+// edge, i.e. "uncertain".
+//
+// Error certificate (u = 2^-24; LEAN_ATAN_ERR_TURNS is what the error bounds charge):
+//   1. the polynomial: |fl(t P(t^2)) - atan(t) / 2pi| <= LEAN_ATAN_POLY_ERR_TURNS for EVERY float t in [0, 1 + 2^-20],
+//      measured exhaustively (tests/cpp/atan_certificate.cu: the Horner chain of lean_atan_poly_turns as compiled,
+//      fmaf = one rounding, against a long double atan; also with the last product t * P left unrounded, which is what a
+//      contraction of p * t into the fold's subtraction would compute);
+//   2. the quotient t = fl(mn * rcp(mx)): MUFU.RCP is within 1 ulp (relative 2^-23 = 2u), the product rounds once (u), so
+//      t = (mn / mx)(1 + eta), |eta| <= 3u + 2u^2, and t <= 1 + 2^-23 (inside the swept range).  atan(t) / 2pi moves by at most
+//      max_t t / (1 + t^2) |eta| / 2pi <= |eta| / 4pi (1 + 1e-6) <= 1.4234e-8 turns.  A denormal t rounds by at most 2^-150
+//      absolutely (nothing in turns).  mx below 2^-126 or above 2^126 makes MUFU.RCP flush to inf / 0: the first gives
+//      NaN / inf downstream, and neither can occur for a point the classifier accepts (n2 > 2e-3 and a finite |p|^2);
+//   3. the octant folds: 0.25 - p lies in [0.124, 0.25] and rounds by at most half an ulp of [2^-3, 2^-2), 2^-27; 0.5 - q
+//      lies in [0.25, 0.5] and rounds by at most 2^-26 (round to nearest; 0.25 and 0.5 are exact).  Both at once: 2.236e-8;
+//   4. copysignf and fabsf, fmaxf, fminf are exact.
+// Sum: LEAN_ATAN_POLY_ERR_TURNS + 1.4234e-8 + 2.236e-8 <= LEAN_ATAN_CERT_TURNS; charged with a margin of about 10 %.
+// coefficients of P, c0 + c1 s + ... + c6 s^6 (scalars: device code may read constexpr scalars, not constexpr arrays)
+constexpr float LEAN_ATAN_C0 = 0.15915432572364807f, LEAN_ATAN_C1 = -0.0530262365937233f, LEAN_ATAN_C2 = 0.03152511641383171f;
+constexpr float LEAN_ATAN_C3 = -0.021061519160866737f, LEAN_ATAN_C4 = 0.012672499753534794f, LEAN_ATAN_C5 = -0.005348276346921921f;
+constexpr float LEAN_ATAN_C6 = 0.0010841299081221223f;
+constexpr double LEAN_ATAN_POLY_ERR_TURNS = 5.31e-8;   // bound of term 1 (the exhaustive sweep measures 5.264e-8)
+constexpr double LEAN_ATAN_QUOT_ERR_TURNS = 1.4234e-8;  // term 2: (3u + 2u^2) / 4pi * (1 + 1e-6), rounded up
+constexpr double LEAN_ATAN_FOLD_ERR_TURNS = 2.2352e-8;  // term 3: 2^-27 + 2^-26, rounded up
+constexpr double LEAN_ATAN_CERT_TURNS = LEAN_ATAN_POLY_ERR_TURNS + LEAN_ATAN_QUOT_ERR_TURNS + LEAN_ATAN_FOLD_ERR_TURNS;
+constexpr double LEAN_ATAN_ERR_TURNS = 1.0e-7;
+static_assert(LEAN_ATAN_ERR_TURNS >= 1.05 * LEAN_ATAN_CERT_TURNS, "the charged arctangent error must cover its certificate");
+
+// P(s), Horner
+VL_HD float lean_atan_horner(float s) {
+  float p = fmaf(s, LEAN_ATAN_C6, LEAN_ATAN_C5);
+  p = fmaf(s, p, LEAN_ATAN_C4);
+  p = fmaf(s, p, LEAN_ATAN_C3);
+  p = fmaf(s, p, LEAN_ATAN_C2);
+  p = fmaf(s, p, LEAN_ATAN_C1);
+  return fmaf(s, p, LEAN_ATAN_C0);
+}
+
+// atan(t) / 2pi for t = mn / mx in [0, 1]: t P(t^2)
+VL_HD float lean_atan_poly_turns(float t) { return lean_atan_horner(t * t) * t; }  // in [0, 1/8]
+
 VL_HD float lean_atan2_turns(float a, float b) {
   const float ax = fabsf(a), bx = fabsf(b);
   const float mx = fmaxf(ax, bx), mn = fminf(ax, bx);
-  const float t = mn * VL_RCPF(mx);
-  const float s = t * t;
-  float p = fmaf(s, 0.0010841299081221223f, -0.005348276346921921f);
-  p = fmaf(s, p, 0.012672499753534794f);
-  p = fmaf(s, p, -0.021061519160866737f);
-  p = fmaf(s, p, 0.03152511641383171f);
-  p = fmaf(s, p, -0.0530262365937233f);
-  p = fmaf(s, p, 0.15915432572364807f);
-  p = p * t;                          // atan(mn / mx) / 2pi in [0, 1/8]
+  float p = lean_atan_poly_turns(mn * VL_RCPF(mx));
   p = ax > bx ? 0.25f - p : p;        // first quadrant
   p = b < 0.0f ? 0.5f - p : p;        // upper half plane
   return copysignf(p, a);
@@ -149,8 +178,9 @@ VL_HD LeanVerdict lean_tail(const LeanCam& c, int width, float up, float vp, flo
 //      (|grad v| <= 2H / 2pi / |p| <= 2H / 2pi / r_xz): eq_lu, eq_lv.  This term is far below the others by construction
 //      (eps / r_xz ~ 1e-7 |dR|): no test can observe it, its charge rests on this derivation alone;
 //   4. the fp32 gradient (relative error <= 16u incl. MUFU.RSQ, charged 64u) times |d| <= r_xz / 16, the products of
-//      g . d, and the rounding of up0 + s at |up| <= 1.03 W + 1 (|s| <= W / 32pi): eq_cu = S (64u W / 32pi + 2u (1.03 W + 1))
-//      + 1e-6 (the reference's own double rounding, the rounding of hx_k), likewise eq_cv with 2H.
+//      g . d, and the rounding of up0 + s, at most u |up0 + s| with |up0| <= W~ / 2 + |cxh~| (make_lean_cam) and
+//      |s| <= W / 32pi: eq_cu = S (64u W / 32pi + u (W~ / 2 + |cxh~| + 0.02 W + 1)) + 1e-6 (the reference's own double
+//      rounding, the rounding of hx_k), likewise eq_cv with 2H~ / 4 + |cyh~| and 2H.
 // m^2 <= (1 + 1/64) |d~|^2 + 65 (eps + sqrt3 delta)^2 (the delta step computes it as fma(|d~|^2, 1.016, e8^2) with
 // e8 = 8.07 (eps + sqrt3 delta)).  Guards at pose k, all from  m < radius  (radius^2 kept per point, shrunk by 1e-4):
 //   * r_xz~ / 16: the remainder bound above; |p_k| >= 15/16 |q0| keeps n^2 > 2e-3 * 0.87 > 1e-3 (the reference's branch);

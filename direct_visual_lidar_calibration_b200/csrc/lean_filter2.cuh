@@ -90,12 +90,12 @@ __device__ __forceinline__ F2 lean_atan2_turns2(F2 a, F2 b) {
   }
   const F2 t = f2_mul(f2_pack(mn[0], mn[1]), f2_pack(LEAN_RCP(mx[0]), LEAN_RCP(mx[1])));
   const F2 s = f2_mul(t, t);
-  F2 p = f2_fma(s, f2_dup(0.0010841299081221223f), -0.005348276346921921f);
-  p = f2_fma(s, p, 0.012672499753534794f);
-  p = f2_fma(s, p, -0.021061519160866737f);
-  p = f2_fma(s, p, 0.03152511641383171f);
-  p = f2_fma(s, p, -0.0530262365937233f);
-  p = f2_fma(s, p, 0.15915432572364807f);
+  F2 p = f2_fma(s, f2_dup(LEAN_ATAN_C6), LEAN_ATAN_C5);  // lean_atan_poly_turns
+  p = f2_fma(s, p, LEAN_ATAN_C4);
+  p = f2_fma(s, p, LEAN_ATAN_C3);
+  p = f2_fma(s, p, LEAN_ATAN_C2);
+  p = f2_fma(s, p, LEAN_ATAN_C1);
+  p = f2_fma(s, p, LEAN_ATAN_C0);
   p = f2_mul(p, t);
   float ps[2];
   f2_unpack(p, ps[0], ps[1]);

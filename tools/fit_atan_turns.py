@@ -1,5 +1,6 @@
 """Fit of the odd minimax polynomial behind lean_atan2_turns (csrc/lean_filter.cuh): atan(t) / 2pi = t P(t^2) on [0, 1], and the
-measured fp32 Horner error of each degree (the kernel uses degree 6 in s = t^2)."""
+measured fp32 Horner error of each degree (the kernel uses degree 6 in s = t^2).  The errors printed here are sampled; the
+bound the classifier charges rests on the exhaustive sweep of tests/cpp/atan_certificate.cu."""
 import numpy as np
 from numpy.polynomial import chebyshev as C
 # fit atan(t)/(2*pi) = t * P(s), s = t^2 on [0,1], minimising max abs error (weighted least squares on Chebyshev nodes, then a few Remez-like reweightings)

@@ -1,0 +1,52 @@
+#!/usr/bin/env python
+"""CPU prediction of the equirectangular deferral rate (tools/, no GPU): the bench.py C3 cloud (uncompressed, not culled)
+at the solves' start poses, each with three poses 1e-3 away (Nelder-Mead's initial simplex), through the host-compiled
+lean classifier (tools/lean_deferral_host.cu): the share of point-poses deferred to the exact path with this tree's
+constants and with those of the looser bound (arctangent charge --other turns, one ulp per FMA rounding), for the plain
+classifier and for the delta step.  Prints one JSON line."""
+import argparse
+import json
+import os
+import shutil
+import subprocess
+import sys
+import tempfile
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--other", type=float, default=2.5e-7, help="arctangent charge to compare with, turns")
+    ap.add_argument("--stride", type=int, default=5, help="every stride-th point per batch")
+    args = ap.parse_args()
+
+    import bench
+    from direct_visual_lidar_calibration_b200 import synthetic as S
+
+    bag = bench.make_inputs(argparse.Namespace(config="C3", points=None), 0)
+    rows = []
+    for T0 in bag["starts"][:8]:
+        batch = [T0] + [S.perturb(T0, tuple(0.057 * np.eye(3)[k]), tuple(1e-3 * np.eye(3)[k])) for k in range(3)]
+        rows.append(np.stack([T[:3, :4].reshape(12) for T in batch]))
+    rows = np.ascontiguousarray(np.stack(rows), dtype=np.float64)
+    pts = np.ascontiguousarray(np.asarray(bag["points"])[:, :3], dtype=np.float32)
+    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+    csrc = os.path.join(ROOT, "direct_visual_lidar_calibration_b200", "csrc")
+    with tempfile.TemporaryDirectory() as tmp:
+        exe, inp = os.path.join(tmp, "lean_deferral_host"), os.path.join(tmp, "in.bin")
+        subprocess.run([nvcc, "-std=c++17", "-O2", "-Wno-deprecated-gpu-targets", "-Xcompiler", "-ffp-contract=off", f"-I{csrc}", f"-I{os.path.join(ROOT, 'include')}", "-o", exe,
+                        os.path.join(ROOT, "tools", "lean_deferral_host.cu")], check=True)
+        with open(inp, "wb") as fh:
+            fh.write(np.array([bag["width"], bag["height"], len(pts), len(rows)], dtype=np.int32).tobytes())
+            fh.write(pts.tobytes())
+            fh.write(rows.tobytes())
+        out = subprocess.run([exe, inp, str(args.stride), repr(args.other)], check=True, capture_output=True, text=True).stdout
+    print(out.strip())
+
+
+if __name__ == "__main__":
+    main()
