@@ -117,7 +117,7 @@ class CostCalculatorNID:
 
     def debug_filter_check(self, Ts, delta=False):
         """Test hook: (point_poses, deferred_to_exact, mismatches, max |uv32-uv64|/bound).  delta: equirectangular delta
-        step -- in every group of 8 poses, pose 0 is the anchor and the others are first-order updates from it."""
+        step -- in every group of 8 poses, the most central pose is the anchor and the others are first-order updates from it."""
         Tc = T_to_colmajor(Ts)
         counts = (C.c_uint64 * 3)()
         ratio = C.c_double()

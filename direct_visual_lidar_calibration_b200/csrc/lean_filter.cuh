@@ -149,13 +149,14 @@ VL_HD LeanVerdict lean_tail(const LeanCam& c, int width, float up, float vp, flo
   return v;
 }
 
-// ---- equirectangular: poses 1..P-1 of a batch as a first-order update from pose 0 (the anchor) -------------------------
+// ---- equirectangular: the poses of a batch as first-order updates from one of them (the anchor) --------------------------
 //
 // The poses of a Nelder-Mead batch lie close together (xr, xe, xc on a line through xo; the initial simplex x0 + 1e-3
 // along each axis), so for pose k the camera-frame point moves by D = p_k - p_0 = dR_k p + dt_k, dR_k = R_k - R_0,
-// dt_k = t_k - t_0, which is small against the point's distance from the camera's y axis r_xz.  The anchor step is the
-// plain classifier at pose 0 (same verdict) and keeps, per point, the projection (up0, vp0), its gradient g at the fp32
-// point q0 = p~_0, 1 / r_xz and a radius within which the guards of the plain classifier provably hold.  The delta step
+// dt_k = t_k - t_0 (index 0: the anchor, lean_delta_anchor), which is small against the point's distance from the
+// camera's y axis r_xz.  The anchor step is the plain classifier at the anchor (same verdict) and keeps, per point, the
+// projection (up0, vp0), its gradient g at the fp32 point q0 = p~_0, 1 / r_xz and a radius within which the guards of the
+// plain classifier provably hold.  The delta step
 // projects pose k as  up = up0 + g_u . d,  vp = vp0 + g_v . d  with d = fl32(dR~_k p + dt~_k) (dR~, dt~ rounded once from
 // the double poses), a handful of FMAs instead of two rsqrt and two arctangents, and keeps the verdict only where
 // |up - u_ref(p_k) + 0.5| < 0.5 - |frac|, i.e. under the half-widths hx_k = hx_0 - (terms 2-4 below), as lean_tail tests.
@@ -164,7 +165,7 @@ VL_HD LeanVerdict lean_tail(const LeanCam& c, int width, float up, float vp, flo
 // p_k and the segment between them.  With xi = p_0 - q0 and h a bound on the Hessian norm of u on B,
 //   u(p_k) - u(p_0) - grad u(q0) . D = int_0^1 (grad u(p_0 + sD) - grad u(q0)) . D ds,  |.| <= h (|xi||D| + |D|^2/2) <= h m^2/2.
 // The error of up splits into
-//   1. the anchor's own bound at pose 0 (0.5 - hx_0: the plain classifier's E, unchanged; hx_0 = hx0 - 1.5 sfx delta / r_xz
+//   1. the anchor's own bound (0.5 - hx_0: the plain classifier's E, unchanged; hx_0 = hx0 - 1.5 sfx delta / r_xz
 //      is recomputed by the delta step in another rounding order, which the safety factor 2 of that term absorbs);
 //   2. the remainder h m^2 / 2.  lon = atan2(x, z) has Hessian norm 1 / r_xz^2.  lat = atan2(y, r_xz(x, z)): its Hessian
 //      is J^T H_2 J + phi_r grad^2 r_xz with J's rows (e_y, grad r_xz) orthonormal, |H_2| = 1 / n^2 (polar angle),
@@ -187,7 +188,7 @@ VL_HD LeanVerdict lean_tail(const LeanCam& c, int width, float up, float vp, flo
 //   * the seam: B must not meet the cut {x = 0, z <= 0} of atan2(x, z): distance r_xz~ if z~ > 0, else |x~|;
 //   * FoV: g = z - cos_fov |p| is 2-Lipschitz and the anchor's margin mf covers its fp32 and the reference's rounding,
 //     so g~_0 - mf > 2|D| keeps the pass at pose k (radius 0.49 (g~_0 - mf)) and -g~_0 - mf > 2|D| keeps the reject.
-// The anchor's own guards (n^2, r_xz > 40 delta, pole) must have held at pose 0 for a pass; otherwise the radius is 0
+// The anchor's own guards (n^2, r_xz > 40 delta, pole) must have held at the anchor for a pass; otherwise the radius is 0
 // and the delta step defers every pose.  A NaN anywhere makes both predicates false: uncertain.
 struct LeanAnchor {
   float up0, vp0;       // the anchor's projection (pixel coordinates minus 0.5)
@@ -201,7 +202,7 @@ struct LeanAnchor {
 constexpr float LEAN_DELTA_SQ3 = 13.98f;   // 8.07 sqrt3
 constexpr float LEAN_DELTA_M2 = 1.016f;    // (1 + 1/64) and the rounding of |d~|^2
 
-// P: pose32 row of pose 0, as classify_lean.  Same operations as the plain classifier for the verdict.
+// P: pose32 row of the anchor, as classify_lean.  Same operations as the plain classifier for the verdict.
 template <int MODEL>
 VL_HD LeanVerdict classify_lean_anchor(const FastCam& f, const LeanCam& c, int width, const float* __restrict__ P, float x, float y, float z, float delta, LeanAnchor& an) {
   static_assert(MODEL == CAM_EQUIRECTANGULAR, "the delta step is derived for the equirectangular model");
@@ -274,10 +275,48 @@ VL_HD LeanVerdict classify_lean_delta(const LeanCam& c, int width, const float* 
 
 // Spread of a batch for the delta step (a performance policy, not part of the bound): beyond it the remainder term would
 // defer too many point-poses, and the batch takes the plain classifier.  Nelder-Mead batches start at ~1e-3 and shrink.
-constexpr double LEAN_DELTA_MAX_DR = 4e-3;  // max |R_k - R_0| entry
-constexpr double LEAN_DELTA_MAX_DT = 2e-2;  // max |t_k - t_0| entry, metres
+constexpr double LEAN_DELTA_MAX_DR = 4e-3;  // max |R_k - R_a| entry (a: the anchor)
+constexpr double LEAN_DELTA_MAX_DT = 2e-2;  // max |t_k - t_a| entry, metres
+constexpr float LEAN_DELTA_T_SCALE = static_cast<float>(LEAN_DELTA_MAX_DR / LEAN_DELTA_MAX_DT);
 
-// pose k of a batch relative to pose 0 (row-major 3x4 doubles) -> Q[16] for classify_lean_delta; true if within the spread
+// gate entry between row r of two poses, fp32 rows [R_r0 R_r1 R_r2 t_r]: the largest |difference|, translation scaled to
+// the rotation's limit (fmaxf: NaN entries are ignored, so a score is never NaN)
+VL_HD float lean_delta_row_spread(const float* __restrict__ a, const float* __restrict__ b) {
+  return fmaxf(fmaxf(fabsf(a[0] - b[0]), fabsf(a[1] - b[1])), fmaxf(fabsf(a[2] - b[2]), LEAN_DELTA_T_SCALE * fabsf(a[3] - b[3])));
+}
+
+// The anchor of a batch of n <= 8 poses (row-major 3x4 doubles; the rule runs on their fp32 roundings): the pose whose
+// largest gate entry to the other poses is smallest, ties to the lowest index, so every block, every rank and the host
+// pick the same pose.  The bound of the delta step holds for any anchor; this choice puts as many batches as possible
+// inside the gate and keeps the remainder term, which grows with the squared distance to the anchor, small.  For a
+// Nelder-Mead iteration {xo, xr, xe, xc} (s = 0, 1, 2, 1/2 along one line) it is xr: the farthest pose is |diff| away
+// instead of 2 |diff|, and the squared offsets sum to 2.25 |diff|^2 instead of 5.25.  For the initial simplex it is x0.
+// pk_delta_rows computes the same scores warp-parallel (max and min are exact, so any grouping gives the same bits).
+VL_HD float lean_delta_anchor_score(const double (*__restrict__ T)[12], int n, int i) {
+  float s = 0.0f;
+  for (int r = 0; r < 3; r++) {
+    float a[4];
+    for (int c = 0; c < 4; c++) a[c] = static_cast<float>(T[i][4 * r + c]);
+    for (int j = 0; j < n; j++) {
+      float b[4];
+      for (int c = 0; c < 4; c++) b[c] = static_cast<float>(T[j][4 * r + c]);
+      s = fmaxf(s, lean_delta_row_spread(a, b));
+    }
+  }
+  return s;
+}
+VL_HD int lean_delta_anchor(const double (*__restrict__ T)[12], int n) {
+  int best = 0;
+  float best_s = n > 0 ? lean_delta_anchor_score(T, n, 0) : 0.0f;
+  for (int i = 1; i < n; i++) {
+    const float s = lean_delta_anchor_score(T, n, i);
+    if (s < best_s) best = i, best_s = s;
+  }
+  return best;
+}
+
+// pose k of a batch relative to the anchor T0 (row-major 3x4 doubles) -> Q[16] for classify_lean_delta (Q[14], Q[15]
+// zero, free for the caller); true if within the spread
 VL_HD bool lean_delta_pose(const double* __restrict__ T, const double* __restrict__ T0, float* __restrict__ Q) {
   float rmax = 0.0f, tmax = 0.0f;
   for (int r = 0; r < 3; r++) {

@@ -398,17 +398,17 @@ int pk_score_poses(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_colma
   bool delta = false;
   if (c0->cam.model == CAM_EQUIRECTANGULAR) {
     const int ch = std::max(1, std::min(PK_MAX_POSES, c0->pk_chunk));
-    auto rows = [&](int p, double* R) {
-      for (int r = 0; r < 3; r++)
-        for (int c = 0; c < 4; c++) R[4 * r + c] = T_colmajor[16 * static_cast<size_t>(p) + r + 4 * c];
-    };
     for (int b = 0; b < n_poses && !delta; b += ch) {
       const int cnt = std::min(ch, n_poses - b);
-      double R0[12], Rk[12];
+      double R[PK_MAX_POSES][12];
+      for (int k = 0; k < cnt; k++)
+        for (int r = 0; r < 3; r++)
+          for (int c = 0; c < 4; c++) R[k][4 * r + c] = T_colmajor[16 * static_cast<size_t>(b + k) + r + 4 * c];
+      const int anc = lean_delta_anchor(R, cnt);  // the kernel's anchor (pk_delta_rows)
       float Q[16];
-      rows(b, R0);
       bool close = cnt >= 2;
-      for (int k = 1; k < cnt && close; k++) rows(b + k, Rk), close = lean_delta_pose(Rk, R0, Q);
+      for (int k = 0; k < cnt && close; k++)
+        if (k != anc) close = lean_delta_pose(R[k], R[anc], Q);
       delta = close;
     }
   }

@@ -55,7 +55,7 @@ constexpr unsigned int PK_TILE_ROWS = 4;
 // Tile ring: every warp streams its tiles through PK_RING shared-memory slots filled by per-lane 16-byte cp.async copies.
 // PK_RING - 1 tiles are in flight; every slot more takes 24 KB of the SM's L1 for shared memory.
 constexpr int PK_RING = 2;
-// Equirectangular batches of nearby poses: poses 1..P-1 as first-order updates from pose 0 (classify_lean2_delta);
+// Equirectangular batches of nearby poses: every pose but the anchor as a first-order update from it (classify_lean2_delta);
 // 0: every pose through the plain classifier (A/B build, `make alt`)
 #ifndef PK_DELTA_POSES
 #define PK_DELTA_POSES 1
@@ -141,7 +141,10 @@ struct PkShared {
   double init_T[16];
   double pose64[PK_MAX_POSES][12];
   float4 pose32[PK_MAX_POSES][4];  // rows: [R00 R01 R02 t0] [R10 R11 R12 t1] [R20 R21 R22 t2] [max|t| 0 0 0]
-  float4 dpose[PK_MAX_POSES][4];   // poses 1..P-1 relative to pose 0, as lean_delta_pose writes them (delta step)
+  // delta step: [1, P) the poses other than the anchor in candidate order, relative to it, as lean_delta_pose writes them,
+  // with .z / .w of row 3 holding the pose's histogram byte offset and its bit of a tile's deferral mask (pk_delta_rows);
+  // [0] holds the anchor: its pose32 rows 0-2 and {index, -, offset, bit}
+  float4 dpose[PK_MAX_POSES][4];
   int delta_on;                    // the batch takes the delta step (block-uniform)
   double ys[PK_MAX_POSES];
   double parts[PK_MAX_WORDS];
@@ -509,14 +512,48 @@ __device__ __forceinline__ void pk_pose_from_list(PkShared& sh, int k, const dou
   sh.pose32[k][3] = make_float4(nextafterf(static_cast<float>(tmax), INFINITY), 0.f, 0.f, 0.f);
 }
 
-// warp 0, once the batch's n poses are in sh.pose64: the rows of the delta step and the batch's gate (every pose within
-// lean_delta_pose's spread of pose 0, and at least two poses)
-__device__ __forceinline__ void pk_delta_rows(PkShared& sh, int n, int lane) {
+static __device__ __noinline__ int pk_delta_anchor(const PkShared& sh, int n, int lane) {
+  // lean_delta_anchor's scores, lane 4i + r taking row r of pose i against every pose, then the lowest-index minimum
+  const int i = lane >> 2, r = lane & 3;
+  float s = 0.0f;
+  if (r < 3 && i < n) {
+    const float4 a = sh.pose32[i][r];
+    for (int j = 0; j < n; j++) {
+      const float4 b = sh.pose32[j][r];
+      s = fmaxf(s, lean_delta_row_spread(&a.x, &b.x));
+    }
+  }
+  s = fmaxf(s, __shfl_xor_sync(0xffffffffu, s, 1));
+  s = fmaxf(s, __shfl_xor_sync(0xffffffffu, s, 2));
+  float m = i < n ? s : INFINITY;
+#pragma unroll
+  for (int o = 4; o < 32; o <<= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  const unsigned int hit = __ballot_sync(0xffffffffu, r == 0 && i < n && s == m);
+  const int anc = hit != 0u ? (__ffs(static_cast<int>(hit)) - 1) >> 2 : 0;
+  return anc;
+}
+
+// warp 0, once the batch's n poses are in sh.pose64 / sh.pose32: the anchor (lean_delta_anchor), the rows of the delta
+// step and the batch's gate (every pose within lean_delta_pose's spread of the anchor, and at least two poses).  K: points
+// per lane of the tile loop (a tile's deferral mask holds bit p * K + j for point j of pose p); nb: bins per histogram.
+template <int K>
+__device__ __forceinline__ void pk_delta_rows(PkShared& sh, int n, int nb, int lane) {
   __syncwarp();
+  const int anc = pk_delta_anchor(sh, n, lane);
+  // lane k in [1, n): the k-th of the other poses in candidate order
   bool close = true;
-  if (lane >= 1 && lane < n) close = lean_delta_pose(sh.pose64[lane], sh.pose64[0], &sh.dpose[lane][0].x);
+  if (lane >= 1 && lane < n) {
+    const int p = lane - (lane <= anc ? 1 : 0);
+    close = lean_delta_pose(sh.pose64[p], sh.pose64[anc], &sh.dpose[lane][0].x);
+    sh.dpose[lane][3].z = __uint_as_float(4u * static_cast<unsigned int>(p * nb));
+    sh.dpose[lane][3].w = __uint_as_float(1u << (p * K));
+  }
   const bool on = __all_sync(0xffffffffu, close) && n >= 2;
-  if (lane == 0) sh.delta_on = on ? 1 : 0;
+  if (lane < 3) sh.dpose[0][lane] = sh.pose32[anc][lane];
+  if (lane == 0) {
+    sh.delta_on = on ? 1 : 0;
+    sh.dpose[0][3] = make_float4(__int_as_float(anc), 0.0f, __uint_as_float(4u * static_cast<unsigned int>(anc * nb)), __uint_as_float(1u << (anc * K)));
+  }
   __syncwarp();
 }
 
@@ -803,9 +840,10 @@ __device__ __forceinline__ void pk_tile(const PkArgs& a, const PkShared& sh, con
     for (int j = 0; j < K; j++)
       if (pend_bin[j] >= 0) red_shared_inc(lb[j] + pend_off + 4u * static_cast<unsigned int>(pend_bin[j]));
   };
-  // the image-bin gathers of pose p's accepted verdicts, consumed by count_previous one pose later
-  auto gather = [&](int p, const bool (&acc)[K], const int (&pix)[K]) {
-    pend_off = 4u * static_cast<unsigned int>(p * a.nb);
+  // the image-bin gathers of a pose's accepted verdicts (off: the byte offset of its histogram), consumed by count_previous
+  // one pose later
+  auto gather = [&](unsigned int off, const bool (&acc)[K], const int (&pix)[K]) {
+    pend_off = off;
 #pragma unroll
     for (int j = 0; j < K; j++) pend_bin[j] = ldg_u8_or_neg(acc[j], B.bin_image + pix[j]);
   };
@@ -818,8 +856,10 @@ __device__ __forceinline__ void pk_tile(const PkArgs& a, const PkShared& sh, con
       pix[j + h] = v.idx[h];
     }
   };
-  // Equirectangular batches whose poses lie close together (sh.delta_on, set with the poses): pose 0 is the anchor, poses
-  // 1..P-1 are first-order updates from it (classify_lean2_delta; bound and guards in lean_filter.cuh)
+  // Equirectangular batches whose poses lie close together (sh.delta_on, set with the poses): the anchor (pk_delta_rows)
+  // goes first through the plain classifier, the other poses are first-order updates from it (classify_lean2_delta; bound
+  // and guards in lean_filter.cuh).  Each row carries its pose's histogram offset and deferral bit, so every count and
+  // every deferral lands in its own pose's slot.
   constexpr bool DELTA = DPOSE && PK_DELTA_POSES && PACKED && MODEL == CAM_EQUIRECTANGULAR;
   const bool delta_tile = DELTA && sh.delta_on;
   if (delta_tile) {
@@ -828,24 +868,30 @@ __device__ __forceinline__ void pk_tile(const PkArgs& a, const PkShared& sh, con
       {
         bool acc[K];
         int pix[K];
-        const float4 r0 = sh.pose32[0][0], r1 = sh.pose32[0][1], r2 = sh.pose32[0][2];
+        const float4 r0 = sh.dpose[0][0], r1 = sh.dpose[0][1], r2 = sh.dpose[0][2], slot = sh.dpose[0][3];
         const float Pm[12] = {r0.x, r0.y, r0.z, r1.x, r1.y, r1.z, r2.x, r2.y, r2.z, r0.w, r1.w, r2.w};
+        unc_bit = __float_as_uint(slot.w);
 #pragma unroll
         for (int j = 0; j < K; j += 2)
           record2(classify_lean2_anchor<MODEL>(a.fast, a.lean, a.width, Pm, X2[j / 2], Y2[j / 2], Z2[j / 2], D2[j / 2], an[j / 2]), j, acc, pix);
-        unc_bit <<= K;
-        gather(0, acc, pix);
+        gather(__float_as_uint(slot.z), acc, pix);
       }
-      for (int p = 1; p < n_poses; p++) {
+      for (int k = 1; k < n_poses; k++) {
         bool acc[K];
         int pix[K];
-        const float4 q0 = sh.dpose[p][0], q1 = sh.dpose[p][1], q2 = sh.dpose[p][2], q3 = sh.dpose[p][3];
+        const float4 q0 = sh.dpose[k][0], q1 = sh.dpose[k][1], q2 = sh.dpose[k][2];
+        const float2 q3 = *reinterpret_cast<const float2*>(&sh.dpose[k][3].x);
         const float Q[14] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, q3.x, q3.y};
+        LeanVerdict2 v[K / 2];
 #pragma unroll
-        for (int j = 0; j < K; j += 2) record2(classify_lean2_delta<MODEL>(a.lean, a.width, Q, X2[j / 2], Y2[j / 2], Z2[j / 2], D2[j / 2], an[j / 2]), j, acc, pix);
-        unc_bit <<= K;
+        for (int j = 0; j < K; j += 2) v[j / 2] = classify_lean2_delta<MODEL>(a.lean, a.width, Q, X2[j / 2], Y2[j / 2], Z2[j / 2], D2[j / 2], an[j / 2]);
+        // the pose's slot, read once its verdicts are in (not held across the classifier)
+        const float2 slot = *reinterpret_cast<const float2*>(&sh.dpose[k][3].z);
+        unc_bit = __float_as_uint(slot.y);
+#pragma unroll
+        for (int j = 0; j < K; j += 2) record2(v[j / 2], j, acc, pix);
         count_previous();
-        gather(p, acc, pix);
+        gather(__float_as_uint(slot.x), acc, pix);
       }
       count_previous();
     }
@@ -873,7 +919,7 @@ __device__ __forceinline__ void pk_tile(const PkArgs& a, const PkShared& sh, con
         unc_bit <<= K;
       }
       count_previous();
-      if (p < n_poses) gather(p, acc, pix);
+      if (p < n_poses) gather(4u * static_cast<unsigned int>(p * a.nb), acc, pix);
     }
   }
   // Deferred (point, pose) pairs of this tile -> the warp's queue for the exact path.  Doing this once per tile instead of inside the pose loop
@@ -1054,13 +1100,13 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
     __syncthreads();
     if (warp == 0) {
       pk_poses_of_candidates(sh, sh.nm.n_cand, lane);
-      if constexpr (DELTA) pk_delta_rows(sh, sh.nm.n_cand, lane);
+      if constexpr (DELTA) pk_delta_rows<K>(sh, sh.nm.n_cand, a.nb, lane);
     }
     if (t == 0) sh.n_poses = sh.nm.n_cand;
   } else {
     const int pc = min(a.chunk, a.n_total);
     if (t < pc) pk_pose_from_list(sh, t, a.poses_in + 12 * static_cast<size_t>(t));  // pc <= 8: warp 0
-    if (DELTA && warp == 0) pk_delta_rows(sh, pc, lane);
+    if (DELTA && warp == 0) pk_delta_rows<K>(sh, pc, a.nb, lane);
     if (t == 0) sh.n_poses = pc;
   }
   for (int i = t; i < PK_MAX_POSES * 2 * PK_MAX_BINS; i += PK_THREADS) (&sh.bmarg[0][0])[i] = 0;
@@ -1215,7 +1261,7 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
       const int pc = static_cast<int>(max(0ll, min(static_cast<long long>(a.chunk), static_cast<long long>(a.n_total) - next0)));
       __syncthreads();
       if (t < pc) pk_pose_from_list(sh, t, a.poses_in + 12 * static_cast<size_t>(next0 + t));
-      if (DELTA && warp == 0) pk_delta_rows(sh, pc, lane);
+      if (DELTA && warp == 0) pk_delta_rows<K>(sh, pc, a.nb, lane);
       if (t == 0) sh.n_poses = pc;
       __syncthreads();
       continue;
@@ -1322,7 +1368,7 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
       }
       const int n_next = sh.nm.n_cand;  // 0 when finished
       pk_poses_of_candidates(sh, n_next, lane);
-      if constexpr (DELTA) pk_delta_rows(sh, n_next, lane);
+      if constexpr (DELTA) pk_delta_rows<K>(sh, n_next, a.nb, lane);
       if (lane == 0) {
         sh.n_poses = n_next;
         sh.tmax = pk_tmax(sh, n_next);
@@ -1364,7 +1410,8 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
 // debug / test kernel: the lean classifier AND the exact path on every (point, pose); a.dbg: [0] point-poses,
 // [1] verdicts deferred to the exact path, [2] kept verdicts that disagree with the exact path (must be 0),
 // [3] max over accepted verdicts of |uv_fp32 - uv_exact| / E as float bits (atomicMax; must stay < 1).
-// DELTA (equirectangular, packed): pose 0 through the anchor step, poses 1..n-1 through the delta step of the hot loop.
+// DELTA (equirectangular, packed): the anchor (lean_delta_anchor) through the anchor step, the other poses through the delta
+// step of the hot loop, whatever their spread.
 template <int MODEL, bool DELTA = false>
 __global__ void __launch_bounds__(NID_THREADS) nid_lean_verify_kernel(const __grid_constant__ NidArgs a, const __grid_constant__ LeanCam lc) {
   const float4* __restrict__ pts = static_cast<const float4*>(a.points);
@@ -1372,8 +1419,11 @@ __global__ void __launch_bounds__(NID_THREADS) nid_lean_verify_kernel(const __gr
   float tmax = 0.f, max_ratio = 0.f;
   for (int p = 0; p < a.n_poses; p++) tmax = fmaxf(tmax, a.pose32[p][12]);
   float Q[NID_MAX_POSES][16];
+  int anc = 0;
   if constexpr (DELTA) {
-    for (int p = 1; p < a.n_poses; p++) lean_delta_pose(a.pose[p], a.pose[0], Q[p]);
+    anc = lean_delta_anchor(a.pose, a.n_poses);
+    for (int p = 0; p < a.n_poses; p++)
+      if (p != anc) lean_delta_pose(a.pose[p], a.pose[anc], Q[p]);
   }
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
   // points in pairs (2k, 2k + 1), as the hot loop classifies them with the packed classifier
@@ -1384,11 +1434,12 @@ __global__ void __launch_bounds__(NID_THREADS) nid_lean_verify_kernel(const __gr
     float delta[2];
     for (int h = 0; h < 2; h++) delta[h] = (5.25f * F32_U) * (fabsf(q2[h].x) + fabsf(q2[h].y) + fabsf(q2[h].z) + tmax);
     LeanAnchor2 an;
-    for (int p = 0; p < a.n_poses; p++) {
+    for (int k = 0; k < a.n_poses; k++) {
+      const int p = k == 0 ? anc : k - (k <= anc ? 1 : 0);  // the anchor first (p == k without the delta step)
       LeanVerdict v2[2];
       if constexpr (DELTA) {
         const F2 X = f2_pack(q2[0].x, q2[1].x), Y = f2_pack(q2[0].y, q2[1].y), Z = f2_pack(q2[0].z, q2[1].z), D = f2_pack(delta[0], delta[1]);
-        const LeanVerdict2 w = p == 0 ? classify_lean2_anchor<MODEL>(a.fast, lc, a.width, a.pose32[0], X, Y, Z, D, an) : classify_lean2_delta<MODEL>(lc, a.width, Q[p], X, Y, Z, D, an);
+        const LeanVerdict2 w = k == 0 ? classify_lean2_anchor<MODEL>(a.fast, lc, a.width, a.pose32[anc], X, Y, Z, D, an) : classify_lean2_delta<MODEL>(lc, a.width, Q[p], X, Y, Z, D, an);
         for (int h = 0; h < 2; h++) {
           v2[h].accept = w.accept[h], v2[h].uncertain = w.uncertain[h], v2[h].idx = w.idx[h];
           v2[h].up = w.up[h], v2[h].vp = w.vp[h], v2[h].hx = w.hx[h], v2[h].hy = w.hy[h];

@@ -203,8 +203,8 @@ int vlcal_nid_reset_profile(vlcal_nid_ctx* ctx);
 /* passes over the cloud since the last reset: a persistent launch (one per inner solve / pose list) carries one pass per
  * Nelder-Mead batch / chunk of 8 poses, a round-1 launch is one pass.  Algorithmic bytes = passes x (16 N + W H). */
 int vlcal_nid_get_profile_passes(vlcal_nid_ctx* ctx, int64_t* passes);
-/* persistent kernel, since the last reset: stats[0] passes whose poses 1..P-1 were classified as first-order updates
- * from pose 0 (equirectangular batches of nearby poses), stats[1] the poses of those passes, stats[2] point-poses
+/* persistent kernel, since the last reset: stats[0] passes whose poses were classified as first-order updates from the
+ * batch's anchor (equirectangular batches of nearby poses), stats[1] the poses of those passes, stats[2] point-poses
  * deferred to the exact fp64 path in the other passes, stats[3] point-poses deferred in the delta passes */
 int vlcal_nid_get_profile_delta(vlcal_nid_ctx* ctx, int64_t stats[4]);
 /* measurement hook: poses carried by one pass over the cloud in pose-list evaluations (vlcal_nid_evaluate /
@@ -244,8 +244,9 @@ int vlcal_nid_filter_enabled(const vlcal_nid_ctx* ctx);
  * counts[1] = verdicts the filter deferred to the exact path, counts[2] = filter verdicts it kept that disagree with the
  * exact path (MUST be 0), *max_bound_ratio = max |uv_fp32 - uv_exact| / error-bound over kept in-image verdicts (< 1). */
 int vlcal_nid_debug_filter_check(vlcal_nid_ctx* ctx, const double* T_camera_lidar, int n_poses, uint64_t counts[3], double* max_bound_ratio);
-/* the same for the equirectangular delta step of the persistent kernel: in every group of 8 poses pose 0 is classified
- * as the anchor and the others as first-order updates from it (whatever their spread) */
+/* the same for the equirectangular delta step of the persistent kernel: in every group of 8 poses the kernel's anchor
+ * (the most central pose) is classified as the anchor and the others as first-order updates from it (whatever their
+ * spread) */
 int vlcal_nid_debug_filter_check_delta(vlcal_nid_ctx* ctx, const double* T_camera_lidar, int n_poses, uint64_t counts[3], double* max_bound_ratio);
 
 /* ---- multi-GPU: fused bag all-reduce over NVLink peer memory ---------------------------------------------------------
