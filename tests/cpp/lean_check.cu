@@ -120,8 +120,106 @@ static void run_case(const Case& cs, unsigned seed, long long n_points, int n_po
   out[0] = total, out[1] = unc, out[2] = mism, out[3] = acc, out[4] = strip, out[6] = static_cast<long long>(max_ratio * 1e6);
 }
 
+// Cone mode: points at angle max_fov (1 +- 10^[-12, -3]) from the optical axis, i.e. inside (and just outside) the
+// uncertain band of the FoV decision (cost_calculator_nid.cpp:32), at an explicit max_fov.  Four poses with small random
+// rotations and translations, as in run_case: the fp32 transform then carries the rounding error the delta terms of the
+// FoV margins bound (a pure translation would leave the camera-frame point nearly exact).  Point i is placed on the cone
+// at pose i % 4 and classified there.
+template <int MODEL>
+static void run_cone(const Case& cs, double fov, unsigned seed, long long n_points, long long out[5]) {
+  CameraParams cam;
+  std::memset(&cam, 0, sizeof(cam));
+  cam.model = MODEL;
+  cam.n_intr = cs.n_intr, cam.n_dist = cs.n_dist;
+  for (int i = 0; i < cs.n_intr; i++) cam.intr[i] = cs.intr[i];
+  for (int i = 0; i < cs.n_dist; i++) cam.dist[i] = cs.dist[i];
+  const FastCam f = make_fast_cam(cam, cs.W, cs.H, fov);
+  const LeanCam lc = make_lean_cam(cam, f, cs.W, cs.H, fov);
+  out[4] = lc.enabled;
+  if (!lc.enabled) return;
+  const double cos_fov = std::cos(fov);
+  std::mt19937_64 rng(seed);
+  std::uniform_real_distribution<double> U(0.0, 1.0);
+  constexpr int n_poses = 4;
+  double poses[12 * n_poses];
+  float poses32[16 * n_poses];
+  float tmax_all = 0.f;
+  for (int p = 0; p < n_poses; p++) {
+    const double xi[6] = {0.05 * (2 * U(rng) - 1), 0.05 * (2 * U(rng) - 1), 0.05 * (2 * U(rng) - 1), 0.3 * (2 * U(rng) - 1), 0.3 * (2 * U(rng) - 1), 0.3 * (2 * U(rng) - 1)};
+    double T[16];
+    host::se3_expmap_gtsam(xi, T);
+    double tm = 0.0;
+    for (int r = 0; r < 3; r++) {
+      for (int c = 0; c < 4; c++) poses[12 * p + 4 * r + c] = T[r + 4 * c];
+      for (int c = 0; c < 3; c++) poses32[16 * p + 3 * r + c] = static_cast<float>(T[r + 4 * c]);
+      poses32[16 * p + 9 + r] = static_cast<float>(T[r + 12]);
+      tm = std::max(tm, std::fabs(T[r + 12]));
+    }
+    poses32[16 * p + 12] = std::nextafter(static_cast<float>(tm), INFINITY);
+    tmax_all = std::max(tmax_all, poses32[16 * p + 12]);
+  }
+  long long unc = 0, mism = 0, inimg = 0;
+  for (long long i = 0; i < n_points; i++) {
+    const int p = static_cast<int>(i % n_poses);
+    const double* P = &poses[12 * p];
+    const double eps = std::pow(10.0, -12.0 + 9.0 * U(rng)) * (U(rng) < 0.5 ? -1 : 1);
+    const double a = fov * (1.0 + eps), az = 2 * M_PI * U(rng), range = 0.5 + 30 * U(rng);
+    // camera-frame point at angle a, moved to the cloud frame: R^T (pc - t)
+    const double pc[3] = {range * std::sin(a) * std::cos(az) - P[3], range * std::sin(a) * std::sin(az) - P[7], range * std::cos(a) - P[11]};
+    const float x = float(P[0] * pc[0] + P[4] * pc[1] + P[8] * pc[2]);
+    const float y = float(P[1] * pc[0] + P[5] * pc[1] + P[9] * pc[2]);
+    const float z = float(P[2] * pc[0] + P[6] * pc[1] + P[10] * pc[2]);
+    const float delta = (5.25f * F32_U) * (std::fabs(x) + std::fabs(y) + std::fabs(z) + tmax_all);
+    const LeanVerdict v = classify_lean<MODEL>(f, lc, cs.W, &poses32[16 * p], x, y, z, delta);
+    double ue, ve;
+    const int pe = exact_pixel_hd<MODEL>(cam, cos_fov, cs.W, cs.H, P, x, y, z, &ue, &ve);
+    if (exact_pixel_hd<MODEL>(cam, -2.0, cs.W, cs.H, P, x, y, z, &ue, &ve) >= 0) inimg++;  // the FoV test left out
+    if (v.uncertain) unc++;
+    else if (v.accept ? v.idx != pe : pe != -1) mism++;
+  }
+  out[0] = n_points, out[1] = unc, out[2] = mism, out[3] = inimg;
+}
+
+static int cone_mode(long long n) {
+  const Case pb = {CAM_PLUMB_BOB, 640, 480, {400, 410, 320, 240, 0}, {-0.04, 0.08, 1e-4, -3e-4, -0.04, 0, 0, 0}, 4, 5};
+  const Case pb0 = {CAM_PLUMB_BOB, 640, 480, {400, 410, 320, 240, 0}, {0, 0, 0, 0, 0, 0, 0, 0}, 4, 5};
+  const Case at = {CAM_ATAN, 640, 480, {400, 400, 320, 240, 0}, {0.9, 0, 0, 0, 0, 0, 0, 0}, 4, 1};
+  const Case rp = {CAM_RATIONAL_POLYNOMIAL, 640, 480, {400, 410, 320, 240, 0}, {-0.04, 0.08, 1e-4, -3e-4, -0.04, 0.01, 0.02, -0.005}, 4, 8};
+  const Case fe = {CAM_FISHEYE, 640, 480, {300, 300, 320, 240, 0}, {0.01, -0.02, 0.003, -0.001, 0, 0, 0, 0}, 4, 4};
+  const Case om = {CAM_OMNIDIR, 640, 480, {300, 300, 320, 240, 1.1}, {-0.1, 0.02, 1e-3, -2e-3, 0, 0, 0, 0}, 5, 4};
+  const Case eq = {CAM_EQUIRECTANGULAR, 640, 320, {640, 320, 0, 0, 0}, {0, 0, 0, 0, 0, 0, 0, 0}, 2, 0};
+  struct ConeCase {
+    const Case* cs;
+    double fov;
+  };
+  // pinhole-type models below their enable threshold cos(max_fov) >= 0.05; the others also beyond 90 degrees
+  const ConeCase cases[] = {{&pb, 0.3}, {&pb, 0.6}, {&pb0, 0.6}, {&at, 0.3}, {&at, 0.6}, {&rp, 0.3}, {&rp, 0.6},
+                            {&fe, 0.5}, {&fe, 0.9}, {&fe, 2.1}, {&om, 0.5}, {&om, 1.2}, {&om, 1.9}, {&eq, 0.5}, {&eq, 1.0}, {&eq, 2.2}};
+  std::printf("[");
+  int k = 0;
+  for (const ConeCase& cc : cases) {
+    long long out[5] = {0, 0, 0, 0, 0};
+    const unsigned seed = 300 + k;
+    switch (cc.cs->model) {
+      case CAM_PLUMB_BOB: run_cone<CAM_PLUMB_BOB>(*cc.cs, cc.fov, seed, n, out); break;
+      case CAM_FISHEYE: run_cone<CAM_FISHEYE>(*cc.cs, cc.fov, seed, n, out); break;
+      case CAM_ATAN: run_cone<CAM_ATAN>(*cc.cs, cc.fov, seed, n, out); break;
+      case CAM_OMNIDIR: run_cone<CAM_OMNIDIR>(*cc.cs, cc.fov, seed, n, out); break;
+      case CAM_EQUIRECTANGULAR: run_cone<CAM_EQUIRECTANGULAR>(*cc.cs, cc.fov, seed, n, out); break;
+      default: run_cone<CAM_RATIONAL_POLYNOMIAL>(*cc.cs, cc.fov, seed, n, out); break;
+    }
+    std::printf("%s{\"case\": %d, \"model\": %d, \"max_fov\": %.3f, \"enabled\": %lld, \"points\": %lld, \"uncertain\": %lld, \"mismatches\": %lld, \"in_image_without_fov\": %lld}",
+                k ? ", " : "", k, cc.cs->model, cc.fov, out[4], out[0], out[1], out[2], out[3]);
+    k++;
+  }
+  std::printf("]\n");
+  return 0;
+}
+
+// argv: [points per case] [mode: 1 edge-adversarial (default), 0 random, 2 FoV cone]
 int main(int argc, char** argv) {
   const long long n = argc > 1 ? std::atoll(argv[1]) : 200000;
+  if (argc > 2 && std::atoi(argv[2]) == 2) return cone_mode(n);
   adversarial = !(argc > 2 && std::atoi(argv[2]) == 0);
   const Case cases[] = {
     // C2 camera (plumb_bob 1920x1080, f = 1000)

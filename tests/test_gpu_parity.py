@@ -433,8 +433,9 @@ FILTER_MODELS = list(util.MODELS)  # every camera model has an fp32 filter with 
 
 
 def _adversarial_problem(model, n, seed):
-    """Clouds that stress the filter's error bound: far points, points skimming the FoV cone and the image border,
-    tiny depths, large lever arms."""
+    """Clouds that stress the filter's error bound: far points (|p| large against the depth, large lever arms) and points
+    very close to the sensor (tiny depths).  Random points almost never fall inside a decision's uncertain band; the FoV
+    cone, the model guards and the pixel edges are targeted in test_gpu_filter_decision_edges.py."""
     rng = np.random.default_rng(seed)
     pr = util.random_problem(model, n=n, seed=seed)
     pts = pr["points"][:, :3].copy()

@@ -2,8 +2,9 @@
 (csrc/exact_classify.cuh; reference decisions: src/vlcal/calib/cost_calculator_nid.cpp:31-38): tests/cpp/lean_check.cu
 is the SAME source the kernel compiles, built host-only.  Every verdict the filter keeps must be the exact path's --
 including the reference's truncation toward zero for u, v in (-1, 0) -- on random and on edge-adversarial points
-(pixel coordinates nudged to within 1e-3 .. 1e-8 px of an integer).  The GPU suite repeats the check with the device
-intrinsics (tests/test_gpu_parity.py::test_filter_error_bound_is_sound)."""
+(pixel coordinates nudged to within 1e-3 .. 1e-8 px of an integer) and on the FoV cone (points at max_fov (1 +- 10^[-12,
+-3]) from the optical axis).  The GPU suite repeats the checks with the device intrinsics
+(tests/test_gpu_parity.py::test_filter_error_bound_is_sound, tests/test_gpu_filter_decision_edges.py)."""
 import json
 import os
 import shutil
@@ -43,3 +44,17 @@ def test_lean_classifier_never_contradicts_the_exact_path(lean_check, adversaria
         assert c["uncertain"] / c["point_poses"] < (0.15 if adversarial else 0.08), c
     # the reference truncates toward zero: u in (-1, 0) is column 0 (cost_calculator_nid.cpp:37) -- the strip must be hit
     assert sum(c["accepted_in_minus_one_strip"] for c in cases if c["model"] == 0) > 100
+
+
+def test_lean_classifier_on_the_fov_cone(lean_check):
+    """Every model at explicit max_fov values where the cone crosses the image, beyond 90 degrees for fisheye, omnidir
+    and equirectangular (cos_fov < 0): no verdict may contradict the exact path, and most of the points must fall inside
+    the uncertain band (otherwise the mode would not reach the decision it is meant to test)."""
+    out = subprocess.run([lean_check, "100000", "2"], check=True, capture_output=True, text=True).stdout
+    cases = json.loads(out)
+    assert len(cases) == 16 and {c["model"] for c in cases} == set(range(6))
+    for c in cases:
+        assert c["enabled"] == 1 and c["points"] == 100000, c
+        assert c["mismatches"] == 0, c
+        assert c["uncertain"] / c["points"] > 0.5, c  # offsets 10^-12 .. 10^-6 of the angle sit inside the band
+        assert c["in_image_without_fov"] / c["points"] > 0.3, c  # the cone crosses the image interior
