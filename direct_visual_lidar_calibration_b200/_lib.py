@@ -164,6 +164,7 @@ def load_library():
     L.vlcal_nid_sweep_max_points.restype = C.c_int64
     L.vlcal_nid_sweep_launch_shape.argtypes = [vp, ip, ip]
     L.vlcal_nid_sweep_last_kernel_ms.restype = C.c_double
+    L.vlcal_nid_debug_sweep_last_deferred.restype = C.c_int64
     L.vlcal_nid_set_poses_per_pass.argtypes = [vp, C.c_int]
     L.vlcal_nid_get_profile_passes.argtypes = [vp, C.POINTER(C.c_int64)]
     L.vlcal_nid_get_profile_delta.argtypes = [vp, C.POINTER(C.c_int64)]

@@ -58,6 +58,7 @@ std::mutex g_sweep_mu;
 std::map<std::pair<int, const void*>, int> g_sweep_occupancy;  // (device, kernel) -> co-resident blocks per SM
 
 thread_local double g_last_kernel_ms = 0.0;
+thread_local long long g_last_deferred = -1;  // of vlcal_nid_debug_sweep_kernel; -1 after the other entry points
 
 // the sweep covers what the persistent kernel covers (float4 clouds, bins <= 32, a camera with the lean classifier, one
 // camera / image size / device for all bags): everything else is refused, and every accepted list can also take the
@@ -123,7 +124,8 @@ int sweep_blocks_per_sm(int device, SweepKernel kernel, int* out) {
 }
 
 // scores of the device pose list d_poses [n_poses][12] -> nid_out (host), bag 0's histograms -> hist_out (host, optional)
-int sweep_launch(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* d_poses, int64_t n_poses, double* nid_out, int32_t* hist_out, int64_t* inliers_out = nullptr) {
+int sweep_launch(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* d_poses, int64_t n_poses, double* nid_out, int32_t* hist_out, int64_t* inliers_out = nullptr,
+                 bool count_deferred = false) {
   vlcal_nid_ctx* c0 = ctxs[0];
   const SweepKernel kernel = sweep_pick(c0->cam.model);
   if (!kernel) {
@@ -139,12 +141,17 @@ int sweep_launch(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* d_poses, 
   const long long groups = (n_poses + SW_POSES - 1) / SW_POSES;
   const int grid = static_cast<int>(std::min<long long>(groups, static_cast<long long>(per_sm) * c0->num_sms));
 
-  DevBuf d_scores, d_hist, d_inl;
-  d_scores.device = d_hist.device = d_inl.device = c0->device;
+  DevBuf d_scores, d_hist, d_inl, d_def;
+  d_scores.device = d_hist.device = d_inl.device = d_def.device = c0->device;
   static_assert(sizeof(long long) == sizeof(int64_t), "inlier counts are copied out as int64_t");
   if (inliers_out) VL_CUDA(MemPool::instance().device_alloc(c0->device, sizeof(long long) * static_cast<size_t>(n_poses), &d_inl.p));
   VL_CUDA(MemPool::instance().device_alloc(c0->device, sizeof(double) * static_cast<size_t>(n_poses), &d_scores.p));
   if (hist_out) VL_CUDA(MemPool::instance().device_alloc(c0->device, sizeof(int) * static_cast<size_t>(n_poses) * nb, &d_hist.p));
+  unsigned long long deferred = 0;
+  if (count_deferred) {
+    VL_CUDA(MemPool::instance().device_alloc(c0->device, sizeof(unsigned long long), &d_def.p));
+    VL_CUDA(cudaMemsetAsync(d_def.p, 0, sizeof(unsigned long long), c0->stream));
+  }
 
   SweepArgs a;
   std::memset(&a, 0, sizeof(a));
@@ -165,6 +172,7 @@ int sweep_launch(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* d_poses, 
   a.scores = static_cast<double*>(d_scores.p);
   a.hist_out = static_cast<int*>(d_hist.p);
   a.inliers = static_cast<long long*>(d_inl.p);
+  a.deferred = static_cast<unsigned long long*>(d_def.p);
 
   EventPair ev;
   VL_CUDA(cudaEventCreate(&ev.start));
@@ -176,7 +184,9 @@ int sweep_launch(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* d_poses, 
   VL_CUDA(cudaMemcpyAsync(nid_out, d_scores.p, sizeof(double) * static_cast<size_t>(n_poses), cudaMemcpyDeviceToHost, c0->stream));
   if (hist_out) VL_CUDA(cudaMemcpyAsync(hist_out, d_hist.p, sizeof(int) * static_cast<size_t>(n_poses) * nb, cudaMemcpyDeviceToHost, c0->stream));
   if (inliers_out) VL_CUDA(cudaMemcpyAsync(inliers_out, d_inl.p, sizeof(int64_t) * static_cast<size_t>(n_poses), cudaMemcpyDeviceToHost, c0->stream));
+  if (count_deferred) VL_CUDA(cudaMemcpyAsync(&deferred, d_def.p, sizeof(deferred), cudaMemcpyDeviceToHost, c0->stream));
   VL_CUDA(cudaStreamSynchronize(c0->stream));
+  g_last_deferred = count_deferred ? static_cast<long long>(deferred) : -1;
   float ms = 0.f;
   VL_CUDA(cudaEventElapsedTime(&ms, ev.start, ev.stop));
   g_last_kernel_ms = ms;
@@ -192,6 +202,7 @@ int sweep_fallback(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_colma
     return VLCAL_ERR_UNSUPPORTED;
   }
   g_last_kernel_ms = 0.0;
+  g_last_deferred = -1;
   return pk_score_poses(ctxs, n_ctxs, T_colmajor, static_cast<int>(n_poses), nid_out, hist_out);
 }
 
@@ -203,6 +214,7 @@ int sweep_fallback_inliers(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double*
     return VLCAL_ERR_UNSUPPORTED;
   }
   g_last_kernel_ms = 0.0;
+  g_last_deferred = -1;
   const size_t nb = static_cast<size_t>(ctxs[0]->bins) * ctxs[0]->bins;
   std::vector<int32_t> hist(static_cast<size_t>(n_poses) * nb);
   std::vector<double> part(static_cast<size_t>(n_poses));
@@ -245,7 +257,7 @@ int sweep_host_list(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_colm
       for (int c = 0; c < 4; c++) hpose[12 * static_cast<size_t>(p) + 4 * r + c] = T[r + 4 * c];
   }
   VL_CUDA(cudaMemcpyAsync(d_poses.p, hpose, pose_bytes, cudaMemcpyHostToDevice, c0->stream));
-  return sweep_launch(ctxs, n_ctxs, static_cast<const double*>(d_poses.p), n_poses, nid_out, hist_out);
+  return sweep_launch(ctxs, n_ctxs, static_cast<const double*>(d_poses.p), n_poses, nid_out, hist_out, nullptr, /*count_deferred=*/!may_fall_back);
 }
 
 int search_set_check(const vlcal_search_set* s) {
@@ -413,5 +425,7 @@ int vlcal_nid_sweep_launch_shape(const vlcal_nid_ctx* ctx, int* blocks, int* pos
 int64_t vlcal_nid_sweep_max_points(void) { return SWEEP_MAX_POINTS; }
 
 double vlcal_nid_sweep_last_kernel_ms(void) { return g_last_kernel_ms; }
+
+int64_t vlcal_nid_debug_sweep_last_deferred(void) { return g_last_deferred; }
 
 }  // extern "C"

@@ -50,6 +50,7 @@ struct SweepArgs {
   double* scores;        // [n_poses]: sum over the bags, in bag order
   int* hist_out;         // optional [n_poses][nb] of bag 0, index = image_bin + lidar_bin*bins
   long long* inliers;    // optional [n_poses]: points counted, summed over the bags (hist_image.sum() of :54)
+  unsigned long long* deferred;  // optional debug count of the (point, pose) pairs sent to the exact path; nullptr: none
 };
 
 struct SweepShared {
@@ -78,6 +79,7 @@ __device__ __forceinline__ void sweep_drain32(const SweepArgs& a, SweepShared& s
     const int pix = exact_pixel_hd<MODEL>(a.cam, a.cos_fov, a.width, a.height, sh.pose64[p], q.x, q.y, q.z);
     if (pix >= 0) atomicAdd(&sh.hist[p][__ldg(B.bin_image + pix) + lidar_bin_of(q.w, a.bins) * a.bins], 1);  // :49
   }
+  if (a.deferred && lane == 0) atomicAdd(a.deferred, static_cast<unsigned long long>(count));
 }
 
 // The NID of one joint histogram in shared memory, by the whole block (cost_calculator_nid.cpp:54-64): the arithmetic and

@@ -172,6 +172,9 @@ int vlcal_nid_sweep_launch_shape(const vlcal_nid_ctx* ctx, int* blocks, int* pos
  * calling thread's last sweep in milliseconds (CUDA events around the kernel; 0 when the persistent kernel ran instead) */
 int vlcal_nid_debug_sweep_kernel(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_camera_lidar, int64_t n_poses, double* nid_out, int32_t* hist_out);
 double vlcal_nid_sweep_last_kernel_ms(void);
+/* debug count of the calling thread's last vlcal_nid_debug_sweep_kernel call: (point, pose) pairs, summed over the
+ * contexts, that the sweep kernel's fp32 filter deferred to the exact path; -1 after any other sweep entry point */
+int64_t vlcal_nid_debug_sweep_last_deferred(void);
 
 /* mode B evaluation with the reference's parameterisation: T_params = P x 7 doubles [qx qy qz qw tx ty tz]
  * (Sophus::SE3d storage, include/vlcal/costs/nid_cost.hpp:38).  ok_out[p] = 0 where the reference functor returns

@@ -122,11 +122,12 @@ static void run_case(const Case& cs, unsigned seed, long long n_points, int n_po
 
 // Cone mode: points at angle max_fov (1 +- 10^[-12, -3]) from the optical axis, i.e. inside (and just outside) the
 // uncertain band of the FoV decision (cost_calculator_nid.cpp:32), at an explicit max_fov.  Four poses with small random
-// rotations and translations, as in run_case: the fp32 transform then carries the rounding error the delta terms of the
-// FoV margins bound (a pure translation would leave the camera-frame point nearly exact).  Point i is placed on the cone
-// at pose i % 4 and classified there.
+// rotations and translations within +-tscale (0.3 m as in run_case; 30 or 300 m for a camera that stands far from the
+// LiDAR origin, as in a map frame, where the max|t| term of delta is a large part of the bound): the fp32 transform then
+// carries the rounding error the delta terms of the FoV margins bound (a pure translation would leave the camera-frame
+// point nearly exact).  Point i is placed on the cone at pose i % 4 and classified there.
 template <int MODEL>
-static void run_cone(const Case& cs, double fov, unsigned seed, long long n_points, long long out[5]) {
+static void run_cone(const Case& cs, double fov, unsigned seed, long long n_points, double tscale, long long out[5]) {
   CameraParams cam;
   std::memset(&cam, 0, sizeof(cam));
   cam.model = MODEL;
@@ -145,7 +146,7 @@ static void run_cone(const Case& cs, double fov, unsigned seed, long long n_poin
   float poses32[16 * n_poses];
   float tmax_all = 0.f;
   for (int p = 0; p < n_poses; p++) {
-    const double xi[6] = {0.05 * (2 * U(rng) - 1), 0.05 * (2 * U(rng) - 1), 0.05 * (2 * U(rng) - 1), 0.3 * (2 * U(rng) - 1), 0.3 * (2 * U(rng) - 1), 0.3 * (2 * U(rng) - 1)};
+    const double xi[6] = {0.05 * (2 * U(rng) - 1), 0.05 * (2 * U(rng) - 1), 0.05 * (2 * U(rng) - 1), tscale * (2 * U(rng) - 1), tscale * (2 * U(rng) - 1), tscale * (2 * U(rng) - 1)};
     double T[16];
     host::se3_expmap_gtsam(xi, T);
     double tm = 0.0;
@@ -180,7 +181,7 @@ static void run_cone(const Case& cs, double fov, unsigned seed, long long n_poin
   out[0] = n_points, out[1] = unc, out[2] = mism, out[3] = inimg;
 }
 
-static int cone_mode(long long n) {
+static int cone_mode(long long n, double tscale) {
   const Case pb = {CAM_PLUMB_BOB, 640, 480, {400, 410, 320, 240, 0}, {-0.04, 0.08, 1e-4, -3e-4, -0.04, 0, 0, 0}, 4, 5};
   const Case pb0 = {CAM_PLUMB_BOB, 640, 480, {400, 410, 320, 240, 0}, {0, 0, 0, 0, 0, 0, 0, 0}, 4, 5};
   const Case at = {CAM_ATAN, 640, 480, {400, 400, 320, 240, 0}, {0.9, 0, 0, 0, 0, 0, 0, 0}, 4, 1};
@@ -201,25 +202,25 @@ static int cone_mode(long long n) {
     long long out[5] = {0, 0, 0, 0, 0};
     const unsigned seed = 300 + k;
     switch (cc.cs->model) {
-      case CAM_PLUMB_BOB: run_cone<CAM_PLUMB_BOB>(*cc.cs, cc.fov, seed, n, out); break;
-      case CAM_FISHEYE: run_cone<CAM_FISHEYE>(*cc.cs, cc.fov, seed, n, out); break;
-      case CAM_ATAN: run_cone<CAM_ATAN>(*cc.cs, cc.fov, seed, n, out); break;
-      case CAM_OMNIDIR: run_cone<CAM_OMNIDIR>(*cc.cs, cc.fov, seed, n, out); break;
-      case CAM_EQUIRECTANGULAR: run_cone<CAM_EQUIRECTANGULAR>(*cc.cs, cc.fov, seed, n, out); break;
-      default: run_cone<CAM_RATIONAL_POLYNOMIAL>(*cc.cs, cc.fov, seed, n, out); break;
+      case CAM_PLUMB_BOB: run_cone<CAM_PLUMB_BOB>(*cc.cs, cc.fov, seed, n, tscale, out); break;
+      case CAM_FISHEYE: run_cone<CAM_FISHEYE>(*cc.cs, cc.fov, seed, n, tscale, out); break;
+      case CAM_ATAN: run_cone<CAM_ATAN>(*cc.cs, cc.fov, seed, n, tscale, out); break;
+      case CAM_OMNIDIR: run_cone<CAM_OMNIDIR>(*cc.cs, cc.fov, seed, n, tscale, out); break;
+      case CAM_EQUIRECTANGULAR: run_cone<CAM_EQUIRECTANGULAR>(*cc.cs, cc.fov, seed, n, tscale, out); break;
+      default: run_cone<CAM_RATIONAL_POLYNOMIAL>(*cc.cs, cc.fov, seed, n, tscale, out); break;
     }
-    std::printf("%s{\"case\": %d, \"model\": %d, \"max_fov\": %.3f, \"enabled\": %lld, \"points\": %lld, \"uncertain\": %lld, \"mismatches\": %lld, \"in_image_without_fov\": %lld}",
-                k ? ", " : "", k, cc.cs->model, cc.fov, out[4], out[0], out[1], out[2], out[3]);
+    std::printf("%s{\"case\": %d, \"model\": %d, \"max_fov\": %.3f, \"translation\": %g, \"enabled\": %lld, \"points\": %lld, \"uncertain\": %lld, \"mismatches\": %lld, \"in_image_without_fov\": %lld}",
+                k ? ", " : "", k, cc.cs->model, cc.fov, tscale, out[4], out[0], out[1], out[2], out[3]);
     k++;
   }
   std::printf("]\n");
   return 0;
 }
 
-// argv: [points per case] [mode: 1 edge-adversarial (default), 0 random, 2 FoV cone]
+// argv: [points per case] [mode: 1 edge-adversarial (default), 0 random, 2 FoV cone] [cone mode: translation scale, m]
 int main(int argc, char** argv) {
   const long long n = argc > 1 ? std::atoll(argv[1]) : 200000;
-  if (argc > 2 && std::atoi(argv[2]) == 2) return cone_mode(n);
+  if (argc > 2 && std::atoi(argv[2]) == 2) return cone_mode(n, argc > 3 ? std::atof(argv[3]) : 0.3);
   adversarial = !(argc > 2 && std::atoi(argv[2]) == 0);
   const Case cases[] = {
     // C2 camera (plumb_bob 1920x1080, f = 1000)

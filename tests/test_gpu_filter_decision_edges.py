@@ -12,7 +12,8 @@ Every case checks
   1. the verify kernels: debug_filter_check reports no verdict that contradicts the exact path, and the fp32 error of
      the accepted verdicts inside the bound (lean classifier, round-1 classifier, and the delta step for equirectangular);
   2. histograms bit-identical to oracle.nid_calculate at the same max_fov (NID within 1e-12) through the persistent
-     kernel, the filter kernel variants 2, 3, 4 and the exact kernel (variant 1);
+     kernel, the filter kernel variants 2, 3, 4, the exact kernel (variant 1) and the pose sweep kernel (K1s, whose
+     scores must also equal the persistent kernel's bit for bit);
   3. that the edge was reached: the oracle confirms the targeted points on the intended side, and the filters defer
      more than a stated share of the targeted point-poses to the exact path.  The count is the cloud's deferred
      point-poses minus those of the same cloud without the targeted points, so the ordinary points' natural deferrals
@@ -23,6 +24,8 @@ import numpy as np
 import pytest
 
 import util
+from direct_visual_lidar_calibration_b200 import _lib
+from direct_visual_lidar_calibration_b200 import initial_guess as ig
 from direct_visual_lidar_calibration_b200 import synthetic as _S
 
 pytestmark = pytest.mark.gpu
@@ -71,12 +74,17 @@ def _refine(pts, q, target, k=3):
     return best, qb
 
 
-def _cone_points(rng, n, fov, eps, T):
-    """n float32 points at angle fov (1 + eps) from the optical axis at pose T (relative offset, oracle's arithmetic)."""
+def _cone_points(rng, n, fov, eps, T, near=None, rg_range=(0.5, 25.0)):
+    """n float32 points at angle fov (1 + eps) from the optical axis at pose T (relative offset, oracle's arithmetic).
+    near = (camera-frame point c on the cone, radius): the points lie within about radius of c instead."""
     a = fov * (1.0 + eps)
-    az = rng.uniform(0.0, 2.0 * math.pi, 4 * n)
-    rg = rng.uniform(0.5, 25.0, 4 * n)
-    pc = np.stack([rg * math.sin(a) * np.cos(az), rg * math.sin(a) * np.sin(az), np.full(4 * n, rg * math.cos(a))], axis=1)
+    if near is None:
+        az = rng.uniform(0.0, 2.0 * math.pi, 4 * n)
+        rg = rng.uniform(*rg_range, 4 * n)
+    else:
+        c = near[0] + rng.uniform(-near[1], near[1], (4 * n, 3))
+        az, rg = np.arctan2(c[:, 1], c[:, 0]), np.linalg.norm(c, axis=1)
+    pc = np.stack([rg * math.sin(a) * np.cos(az), rg * math.sin(a) * np.sin(az), rg * math.cos(a)], axis=1)
     q = lambda p: np.arccos(np.clip(_nz(T, p), -1.0, 1.0)) / fov - 1.0
     pts, got = _refine(_to_cloud(T, pc), q, eps)
     keep = np.argsort(np.abs(got - eps), kind="stable")[:n]  # the best quarter of the candidates
@@ -149,7 +157,16 @@ def _deferred(V, pr, Ts, max_fov, delta):
     cost.calculate_batch(Ts)
     prof = cost.profile()
     out["persistent"] = prof["deferred_plain"] + prof["deferred_delta"]
+    out["sweep"] = _sweep(cost, Ts)[2]
     return out
+
+
+def _sweep(cost, Ts):
+    """The pose sweep kernel on Ts whatever the cloud size: (NID, histograms, (point, pose) pairs it deferred)."""
+    nid, hist = ig.sweep_poses([cost], Ts, return_hist=True, kernel_only=True)
+    deferred = int(_lib.load_library().vlcal_nid_debug_sweep_last_deferred())
+    assert deferred >= 0
+    return nid, hist, deferred
 
 
 def _check(V, O, pr, Ts, max_fov=None, at=None, n_band=0, floor=0.5, name=""):
@@ -184,13 +201,20 @@ def _check(V, O, pr, Ts, max_fov=None, at=None, n_band=0, floor=0.5, name=""):
     _assert_nid(nid, ref_nid)
     out["persistent"] = prof["deferred_plain"] + prof["deferred_delta"]
     out["delta_passes"] = prof["delta_passes"]
+    pk_nid = nid
     for variant in (2, 3, 4, 1):
         cost.set_kernel_variant(variant)
         nid, hist = cost.calculate_batch(Ts, return_hist=True)
         assert np.array_equal(hist, ref_hist), (name, variant, int(np.abs(hist.astype(np.int64) - ref_hist).sum()))
         _assert_nid(nid, ref_nid)
+    cost.set_kernel_variant(0)
+    # K1s: groups of 4 poses, its own copy of the bound and its own deferral queue
+    nid, hist, out["sweep"] = _sweep(cost, Ts)
+    assert np.array_equal(hist, ref_hist), (name, "sweep", int(np.abs(hist.astype(np.int64) - ref_hist).sum()))
+    _assert_nid(nid, ref_nid)
+    assert np.array_equal(nid, pk_nid, equal_nan=True), name
     # 3. the edge was reached: deferrals of the targeted points, over those of the same cloud without them
-    keys = ("lean", "round1", "persistent") + (("delta",) if delta else ())
+    keys = ("lean", "round1", "persistent", "sweep") + (("delta",) if delta else ())
     if n_band:
         base = _deferred(V, dict(pr, points=np.delete(pr["points"], at, axis=0), intensities=np.delete(pr["intensities"], at)), Ts, max_fov, delta)
         for key in keys:
@@ -334,28 +358,34 @@ def _direction_for_pixel(O, cam, uv, z):
     return np.c_[xy * z[:, None], z]
 
 
-def _equirect_points(W, H, uv, rng):
+def _equirect_points(W, H, uv, rng, rg_range=(0.5, 25.0)):
     """Inverse of equirectangular.hpp:21-27: lon = atan2(x, z), lat = -asin(y / |p|)."""
     lon = (uv[:, 0] / W - 0.5) * 2.0 * math.pi
     lat = (0.5 - uv[:, 1] / H) * math.pi
-    rg = rng.uniform(0.5, 25.0, len(uv))
+    rg = rng.uniform(*rg_range, len(uv))
     return np.stack([rg * np.cos(lat) * np.sin(lon), -rg * np.sin(lat), rg * np.cos(lat) * np.cos(lon)], axis=1)
 
 
-def _edge_points(O, cam, pr0, T, axis, off, n, tol, rng, strips=True):
+def _edge_points(O, cam, pr0, T, axis, off, n, tol, rng, strips=True, z_range=(1.0, 20.0), near=None):
     """n float32 points whose oracle coordinate `axis` at pose T lies within tol of an integer edge + off: interior
-    edges, and with strips=True also 0 and -1 (the (-1, 0) truncation strip) and W / H.  -> (points, their edges)."""
+    edges, and with strips=True also 0 and -1 (the (-1, 0) truncation strip) and W / H.  Depth (equirectangular: range)
+    in z_range; near = (pixel, spread): only edges and pixels within spread px of it.  -> (points, their edges)."""
     W, H = pr0["W"], pr0["H"]
     m = 4 * n  # candidates
-    edge = rng.integers(1, (W if axis == 0 else H), m).astype(np.float64)
-    if strips:
-        edge[:20], edge[20:40], edge[40:60] = 0.0, -1.0, (W if axis == 0 else H)
-    uv = np.stack([rng.uniform(5.0, W - 5.0, m), rng.uniform(5.0, H - 5.0, m)], axis=1)
+    if near is None:
+        edge = rng.integers(1, (W if axis == 0 else H), m).astype(np.float64)
+        if strips:
+            edge[:20], edge[20:40], edge[40:60] = 0.0, -1.0, (W if axis == 0 else H)
+        uv = np.stack([rng.uniform(5.0, W - 5.0, m), rng.uniform(5.0, H - 5.0, m)], axis=1)
+    else:
+        s = int(near[1])
+        edge = np.floor(near[0][axis]) + rng.integers(-s, s + 2, m)
+        uv = near[0] + rng.uniform(-near[1], near[1], (m, 2))
     uv[:, axis] = edge + off
     if pr0["model"] == "equirectangular":
-        pc = _equirect_points(W, H, uv, rng)
+        pc = _equirect_points(W, H, uv, rng, z_range)
     else:
-        pc = _direction_for_pixel(O, cam, uv, rng.uniform(1.0, 20.0, m))
+        pc = _direction_for_pixel(O, cam, uv, rng.uniform(*z_range, m))
     q = lambda p: O.project(cam, _camera_frame(T, p))[:, axis] - (edge + off)
     pts, got = _refine(_to_cloud(T, pc), q, 0.0)
     ok = np.abs(got) <= tol  # got: distance from the targeted offset, px (NaN: Newton did not converge)
@@ -631,3 +661,181 @@ def test_delta_step_at_the_cone(gpu, oracle):
     pr["T"] = T0
     out = _check(gpu, oracle, pr, Ts, max_fov=fov, at=at, n_band=n_band, name="delta step at the cone")
     assert out["delta_passes"] == 1, out
+
+
+# ---- 6. large translations: the max|t| term of the bound -------------------------------------------------------------------
+#
+# Every fp32 filter bounds the transform error of a point by delta = 5.25 u (|x| + |y| + |z| + max|t|), max|t| over the
+# poses that share the bound (a K1p pass, a K1s group, a round-1 pose).  Two geometries make that term matter:
+#   (a) a far camera over a near cloud: |t| of 30 and 300 m, the points within about 1 m of the LiDAR origin, so
+#       max|t| is nearly all of delta;
+#   (b) the map frame (preprocess_map keeps the map's coordinates): points 60 and 450 m from the origin and the camera
+#       among them, where R p and t cancel.
+# Each translation is moved to about half a float32 ulp from its float32 value, on the side where that rounding pushes
+# the targeted points down across their edges.  The pose of largest |t| stands first, in the middle and last of a K1p
+# pass and a round-1 launch of 8 poses and of a K1s group of 4, the other one in other slots, among ordinary poses.
+
+FAR_SLOTS = ((0, 0), (13, 0), (23, 0), (5, 1), (18, 1))  # (index in a list of 24 poses, which large-|t| pose)
+FAR_DIST = (300.0, 30.0)  # (a): distance of the LiDAR origin from the camera, largest first
+MAP_DIST = (450.0, 60.0)  # (b): distance of the camera from the map origin, largest first
+FAR_EDGE_OFFSETS = [1e-5, 3e-6, 1e-6, -1e-6]  # px
+MAP_EDGE_OFFSETS = {450.0: [1e-3, -1e-3], 60.0: [1e-4, -1e-4]}  # px: the float32 grid of the cloud is coarser there
+MAP_CONE_OFFSETS = {450.0: [1e-5, -1e-5, 3e-6], 60.0: [3e-6, -3e-6, 1e-6]}  # relative, in angle
+
+
+def _push_translation(T, qc, pc0):
+    """T with every translation component set to about half a float32 ulp from its float32 value, on the side where
+    float32(t) lowers the camera-frame quantity qc at pc0."""
+    T = T.copy()
+    for k in range(3):
+        e = np.zeros((1, 3))
+        e[0, k] = 1e-4 * np.linalg.norm(pc0)
+        g = float(qc(pc0[None] + e)[0] - qc(pc0[None] - e)[0])
+        f = np.float32(T[k, 3])
+        T[k, 3] = float(f) + math.copysign(0.49, g) * float(np.spacing(np.abs(f)))
+        assert np.float32(T[k, 3]) == f
+    return T
+
+
+def _with_large_poses(T0, large, seed):
+    """24 poses around T0 with the large-|t| poses at FAR_SLOTS."""
+    Ts = util.random_poses(T0, 24, seed=seed)
+    for i, k in FAR_SLOTS:
+        Ts[i] = large[k]
+    return Ts
+
+
+def _n_slots(k):
+    return sum(1 for _, j in FAR_SLOTS if j == k)
+
+
+def _angle_q(fov):
+    return lambda pc: np.arccos(np.clip(pc[:, 2] / np.linalg.norm(pc, axis=1), -1.0, 1.0)) / fov - 1.0
+
+
+def _cone_direction_in_image(O, cam, pr0, fov):
+    """A unit camera-frame direction at angle fov from the axis that lands in the image (the FoV test left out)."""
+    for az in np.linspace(0.0, 2.0 * math.pi, 97)[:-1]:
+        d = np.array([math.sin(fov) * math.cos(az), math.sin(fov) * math.sin(az), math.cos(fov)])
+        uv = O.project(cam, d[None])[0]
+        if np.all(np.isfinite(uv)) and 0.0 <= uv[0] < pr0["W"] and 0.0 <= uv[1] < pr0["H"]:
+            return d
+    raise AssertionError("the cone misses the image")
+
+
+def _pixel_direction(O, cam, pr0, uv, dist):
+    """The camera-frame point of pixel uv at depth dist (equirectangular: range), as _edge_points places them."""
+    if pr0["model"] == "equirectangular":
+        return _equirect_points(pr0["W"], pr0["H"], uv[None], np.random.default_rng(0), (dist, dist))[0]
+    return _direction_for_pixel(O, cam, uv[None], np.array([dist]))[0]
+
+
+def _large_pose(T0, pc_origin):
+    """T0's rotation with the LiDAR origin at camera-frame point pc_origin."""
+    T = T0.copy()
+    T[:3, 3] = pc_origin
+    return T
+
+
+def _map_pose(T0, C):
+    """T0's rotation with the camera at LiDAR-frame (map) position C."""
+    T = T0.copy()
+    T[:3, 3] = -T0[:3, :3] @ C
+    return T
+
+
+@pytest.mark.parametrize("model", util.MODELS)
+def test_far_camera_near_cloud_at_the_cone(gpu, oracle, model):
+    """(a) at the cone: the LiDAR origin on the cone of the widest max_fov of the model, 300 and 30 m away; the targeted
+    points within about 1 m of it, at the offsets of section 1."""
+    rng = np.random.default_rng(200 + len(model))
+    pr0 = util.random_problem(model, n=16)
+    cam, _ = _oracle_fov(oracle, pr0)
+    fov = CONE_FOVS[model][-1]
+    d = _cone_direction_in_image(oracle, cam, pr0, fov)
+    groups, n_band, large = [], 0, []
+    for k, dist in enumerate(FAR_DIST):
+        T = _push_translation(_large_pose(pr0["T"], dist * d), _angle_q(fov), dist * d)
+        large.append(T)
+        for eps in CONE_OFFSETS:
+            pts, got = _cone_points(rng, 300, fov, eps, T, near=(T[:3, 3], 1.0))
+            _assert_placed(got, eps)
+            assert np.abs(pts).max() < 2.0
+            groups.append(pts)
+            n_band += _n_slots(k) * len(pts) if abs(eps) <= IN_BAND else 0
+    pr, at = _problem(model, np.concatenate(groups), seed=201)
+    _check(gpu, oracle, pr, _with_large_poses(pr0["T"], large, seed=202), max_fov=fov, at=at, n_band=n_band, name=f"{model} far cone")
+
+
+@pytest.mark.parametrize("model", util.MODELS)
+def test_far_camera_near_cloud_at_pixel_edges(gpu, oracle, model):
+    """(a) at the pixel edges: the LiDAR origin 300 and 30 m away in front of the image centre; targeted points within
+    1e-5 ... 1e-6 px of the columns and rows about its pixel, within about 1 m of it."""
+    rng = np.random.default_rng(210 + len(model))
+    pr0 = util.random_problem(model, n=16)
+    cam, _ = _oracle_fov(oracle, pr0)
+    uv_c = np.array([0.5 * pr0["W"] + 37.3, 0.5 * pr0["H"] - 23.7])
+    groups, n_band, large = [], 0, []
+    for k, dist in enumerate(FAR_DIST):
+        pc0 = _pixel_direction(oracle, cam, pr0, uv_c, dist)
+        spread = float(np.abs(oracle.project(cam, pc0[None] + [0.5, 0.0, 0.0]) - uv_c).max())  # px of 0.5 m there
+        T = _push_translation(_large_pose(pr0["T"], pc0), lambda pc, a=k % 2: oracle.project(cam, pc)[:, a], pc0)
+        large.append(T)
+        for axis in (0, 1):
+            for off in FAR_EDGE_OFFSETS:
+                pts, _ = _edge_points(oracle, cam, pr0, T, axis, off, 150, 0.3 * abs(off), rng, z_range=(dist - 0.7, dist + 0.7), near=(uv_c, spread))
+                assert np.abs(pts).max() < 3.0
+                groups.append(pts)
+                n_band += _n_slots(k) * len(pts)
+    pr, at = _problem(model, np.concatenate(groups), seed=211)
+    _check(gpu, oracle, pr, _with_large_poses(pr0["T"], large, seed=212), at=at, n_band=n_band, name=f"{model} far pixel edges")
+
+
+@pytest.mark.parametrize("model", util.MODELS)
+def test_map_frame_cone_and_pixel_edges(gpu, oracle, model):
+    """(b): the camera 450 and 60 m from the map origin, the targeted points 15-25 m from it: on the cone (its widest
+    max_fov) in one case, on pixel edges (the estimated max_fov) in the other.  Then a whole map-frame cloud: the
+    share of point-poses the filters defer there."""
+    rng = np.random.default_rng(220 + len(model))
+    pr0 = util.random_problem(model, n=16)
+    cam, _ = _oracle_fov(oracle, pr0)
+    fov = CONE_FOVS[model][-1]
+    direction = np.array([0.48, -0.6, 0.64])
+    uv_c = np.array([0.5 * pr0["W"] + 37.3, 0.5 * pr0["H"] - 23.7])
+    d = _cone_direction_in_image(oracle, cam, pr0, fov)
+    for kind in ("cone", "pixel"):
+        groups, n_band, large = [], 0, []
+        for k, dist in enumerate(MAP_DIST):
+            T = _map_pose(pr0["T"], dist * direction)
+            if kind == "cone":
+                T = _push_translation(T, _angle_q(fov), 20.0 * d)
+            else:
+                pc0 = _pixel_direction(oracle, cam, pr0, uv_c, 20.0)
+                T = _push_translation(T, lambda pc, a=k % 2: oracle.project(cam, pc)[:, a], pc0)
+            large.append(T)
+            if kind == "cone":
+                for eps in MAP_CONE_OFFSETS[dist]:
+                    pts, got = _cone_points(rng, 300, fov, eps, T, rg_range=(15.0, 25.0))
+                    _assert_placed(got, eps)
+                    groups.append(pts)
+                    n_band += _n_slots(k) * len(pts)
+            else:
+                for axis in (0, 1):
+                    for off in MAP_EDGE_OFFSETS[dist]:
+                        pts, _ = _edge_points(oracle, cam, pr0, T, axis, off, 150, 0.3 * abs(off), rng, z_range=(15.0, 25.0), near=(uv_c, 100.0))
+                        groups.append(pts)
+                        n_band += _n_slots(k) * len(pts)
+            assert np.median(np.linalg.norm(groups[-1], axis=1)) > 0.5 * dist
+        pr, at = _problem(model, np.concatenate(groups), seed=221)
+        _check(gpu, oracle, pr, _with_large_poses(pr0["T"], large, seed=222), max_fov=fov if kind == "cone" else None, at=at, n_band=n_band,
+               name=f"{model} map frame {kind}")
+    # a whole cloud in the map frame, seen from its own camera: no targets, the deferred share is reported
+    pr = util.random_problem(model, n=20_000, seed=223)
+    C = MAP_DIST[0] * direction
+    pr["points"][:, :3] = (pr["points"][:, :3] + C).astype(np.float32).astype(np.float64)
+    Ts = util.random_poses(pr["T"], 8, seed=224)
+    Ts[:, :3, 3] -= np.einsum("nij,j->ni", Ts[:, :3, :3], C)  # the same cameras relative to the moved cloud
+    out = _check(gpu, oracle, pr, Ts, name=f"{model} map-frame cloud")
+    n_pp = len(pr["points"]) * len(Ts)
+    print(f"{model} map-frame cloud at {MAP_DIST[0]:g} m: deferred share lean {out['lean'] / n_pp:.4f}, persistent {out['persistent'] / n_pp:.4f}, "
+          f"sweep {out['sweep'] / n_pp:.4f}")

@@ -46,11 +46,8 @@ def test_lean_classifier_never_contradicts_the_exact_path(lean_check, adversaria
     assert sum(c["accepted_in_minus_one_strip"] for c in cases if c["model"] == 0) > 100
 
 
-def test_lean_classifier_on_the_fov_cone(lean_check):
-    """Every model at explicit max_fov values where the cone crosses the image, beyond 90 degrees for fisheye, omnidir
-    and equirectangular (cos_fov < 0): no verdict may contradict the exact path, and most of the points must fall inside
-    the uncertain band (otherwise the mode would not reach the decision it is meant to test)."""
-    out = subprocess.run([lean_check, "100000", "2"], check=True, capture_output=True, text=True).stdout
+def _check_cone(lean_check, *translation):
+    out = subprocess.run([lean_check, "100000", "2", *translation], check=True, capture_output=True, text=True).stdout
     cases = json.loads(out)
     assert len(cases) == 16 and {c["model"] for c in cases} == set(range(6))
     for c in cases:
@@ -58,3 +55,17 @@ def test_lean_classifier_on_the_fov_cone(lean_check):
         assert c["mismatches"] == 0, c
         assert c["uncertain"] / c["points"] > 0.5, c  # offsets 10^-12 .. 10^-6 of the angle sit inside the band
         assert c["in_image_without_fov"] / c["points"] > 0.3, c  # the cone crosses the image interior
+
+
+def test_lean_classifier_on_the_fov_cone(lean_check):
+    """Every model at explicit max_fov values where the cone crosses the image, beyond 90 degrees for fisheye, omnidir
+    and equirectangular (cos_fov < 0): no verdict may contradict the exact path, and most of the points must fall inside
+    the uncertain band (otherwise the mode would not reach the decision it is meant to test)."""
+    _check_cone(lean_check)
+
+
+@pytest.mark.parametrize("translation", ["30", "300"])
+def test_lean_classifier_on_the_fov_cone_far_from_the_lidar_origin(lean_check, translation):
+    """The cone cases with pose translations up to 30 and 300 m: the camera stands far from the LiDAR origin, as in a
+    map frame, and the max|t| term is a large part of the bound."""
+    _check_cone(lean_check, translation)
