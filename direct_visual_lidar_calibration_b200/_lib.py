@@ -149,6 +149,7 @@ def load_library():
     L.vlcal_camera_project.argtypes = [C.c_int, dp, C.c_int, dp, C.c_int, dp, dp]
     L.vlcal_se3_expmap_gtsam.argtypes = [dp, dp]
     L.vlcal_estimate_camera_fov.argtypes = [C.c_int, dp, C.c_int, dp, C.c_int, C.c_int, C.c_int, dp]
+    L.vlcal_outer_step_delta.argtypes = [dp, dp, dp, dp]
     L.vlcal_nid_create.argtypes = [C.POINTER(vp), C.c_int, C.c_int, C.c_int, dp, C.c_int, dp, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int64, C.c_int, C.c_double]
     L.vlcal_nid_destroy.argtypes = [vp]
     L.vlcal_nid_destroy.restype = None

@@ -34,6 +34,14 @@ def estimate_camera_fov(proj: GenericCamera, image_size) -> float:
     return float(out.value)
 
 
+def outer_step_delta(T, new_T):
+    """(delta_t, delta_r) of the outer loop (visual_camera_calibration.cpp:50-54): new_T^-1 * T as isometries, its
+    translation norm and AngleAxisd angle -- the same bits the Nelder-Mead branch's outer loop decides on."""
+    dt, dr = C.c_double(), C.c_double()
+    _lib.check(_lib.load_library().vlcal_outer_step_delta(_dp(T_to_colmajor(T)), _dp(T_to_colmajor(new_T)), C.byref(dt), C.byref(dr)))
+    return float(dt.value), float(dr.value)
+
+
 class VisualCameraCalibrationParams:
     def __init__(self):  # visual_camera_calibration.hpp:12-26
         self.max_outer_iterations = 10
@@ -148,10 +156,8 @@ class VisualCameraCalibration:
         for _ in range(self.params.max_outer_iterations):
             new_T, r = self.estimate_pose_bfgs(T)
             inner.append(r)
-            delta = np.linalg.inv(new_T) @ T
+            delta_t, delta_r = outer_step_delta(T, new_T)
             T = new_T
-            delta_t = float(np.linalg.norm(delta[:3, 3]))
-            delta_r = float(np.arccos(np.clip(0.5 * (np.trace(delta[:3, :3]) - 1.0), -1.0, 1.0)))
             if delta_t < self.params.delta_trans_thresh and delta_r < self.params.delta_rot_thresh:
                 break
         self.stats = {"outer_iterations": len(inner), "inner": inner, "total_evaluations": sum(r["evaluations"] for r in inner)}

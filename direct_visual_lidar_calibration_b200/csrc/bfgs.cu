@@ -242,6 +242,7 @@ extern "C" int vlcal_bfgs_minimize_se3(
   if (!cur.valid) {
     set_last_error("the objective cannot be evaluated at the initial pose");
     res.termination = VLCAL_BFGS_FAILURE;
+    res.evaluations = S.evaluations;
     if (result) *result = res;
     std::memcpy(T_out, init_T, 16 * sizeof(double));
     return VLCAL_OK;

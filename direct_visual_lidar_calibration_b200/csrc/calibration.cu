@@ -355,6 +355,16 @@ int check_common(const vlcal_calib_params* params, const double* init_T, double*
   return VLCAL_OK;
 }
 
+// visual_camera_calibration.cpp:50-54: delta = new_T^-1 * T, its translation norm and its rotation angle
+void outer_step_delta(const double T[16], const double new_T[16], double* delta_t, double* delta_r) {
+  double inv[16], delta[16];
+  host::isometry_inverse(new_T, inv);
+  host::isometry_mul(inv, T, delta);  // :50
+  const double tx = host::m4(delta, 0, 3), ty = host::m4(delta, 1, 3), tz = host::m4(delta, 2, 3);
+  *delta_t = std::sqrt((tx * tx + ty * ty) + tz * tz);  // :53
+  *delta_r = host::rotation_angle(delta);               // :54
+}
+
 }  // namespace
 
 void vlcal::solve_trace_clear() {
@@ -552,18 +562,23 @@ int vlcal_calibrate_nelder_mead(
     double new_T[16];
     rc = inner_solve_resident(device, cam, resident, params, T, callback, allreduce, user, profiling, new_T, nullptr, stats, i);  // :46
     if (rc != VLCAL_OK) return rc;
-    double inv[16], delta[16];
-    host::isometry_inverse(new_T, inv);
-    host::isometry_mul(inv, T, delta);  // :50
-    std::memcpy(T, new_T, sizeof(T));   // :51
-    const double tx = host::m4(delta, 0, 3), ty = host::m4(delta, 1, 3), tz = host::m4(delta, 2, 3);
-    const double delta_t = std::sqrt((tx * tx + ty * ty) + tz * tz);  // :53
-    const double delta_r = host::rotation_angle(delta);               // :54
+    double delta_t, delta_r;
+    outer_step_delta(T, new_T, &delta_t, &delta_r);
+    std::memcpy(T, new_T, sizeof(T));  // :51
     const bool converged = delta_t < params->delta_trans_thresh && delta_r < params->delta_rot_thresh;  // :55
     if (stats) stats->outer_iterations = i + 1;
     if (converged) break;  // :62-64
   }
   std::memcpy(T_out, T, sizeof(T));
+  return VLCAL_OK;
+}
+
+int vlcal_outer_step_delta(const double T_colmajor[16], const double new_T_colmajor[16], double* delta_t, double* delta_r) {
+  if (!T_colmajor || !new_T_colmajor || !delta_t || !delta_r) {
+    set_last_error("NULL argument");
+    return VLCAL_ERR_INVALID_ARGUMENT;
+  }
+  outer_step_delta(T_colmajor, new_T_colmajor, delta_t, delta_r);
   return VLCAL_OK;
 }
 

@@ -557,6 +557,11 @@ int vlcal_calibrate_nelder_mead(
   double T_out[16],
   vlcal_calib_stats* stats);
 
+/* the outer loop's step size (visual_camera_calibration.cpp:50-54): delta = new_T^-1 * T as isometries,
+ * delta_t = |delta.translation()|, delta_r = AngleAxisd(delta.linear()).angle().  Both branches' outer loops stop on
+ * delta_t < delta_trans_thresh && delta_r < delta_rot_thresh with these values. */
+int vlcal_outer_step_delta(const double T_colmajor[16], const double new_T_colmajor[16], double* delta_t, double* delta_r);
+
 /* ---- NID_BFGS branch (VisualCameraCalibration::estimate_pose_bfgs, visual_camera_calibration.cpp:187-238) -------------
  * The reference solves min_T sum_bags NIDCost(T) with ceres::GradientProblemSolver (line-search BFGS) on the
  * Sophus::Manifold<SE3>.  Ceres is not available to this build, so this is a Ceres-free BFGS with the same problem

@@ -6,6 +6,7 @@ import this module.  The product package (direct_visual_lidar_calibration_b200) 
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 import subprocess
 
@@ -182,9 +183,21 @@ def isometry_mul(A, B) -> np.ndarray:
     return colmajor_to_T(c)
 
 
+def isometry_inverse(A) -> np.ndarray:
+    a, b = T_to_colmajor(A), np.empty(16)
+    lib().orc_isometry_inverse(_dp(a), _dp(b))
+    return colmajor_to_T(b)
+
+
 def rotation_angle(T) -> float:
     a = T_to_colmajor(T)
     return float(lib().orc_rotation_angle(_dp(a)))
+
+
+def outer_step_delta(T, new_T):
+    """(delta_t, delta_r) of orc_calibrate's outer loop (visual_camera_calibration.cpp:50-54)."""
+    d = isometry_mul(isometry_inverse(new_T), T)
+    return math.sqrt((d[0, 3] * d[0, 3] + d[1, 3] * d[1, 3]) + d[2, 3] * d[2, 3]), rotation_angle(d)
 
 
 def estimate_camera_fov(cam: Camera, width: int, height: int) -> float:

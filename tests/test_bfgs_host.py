@@ -7,6 +7,7 @@ from scipy.spatial.transform import Rotation
 
 import direct_visual_lidar_calibration_b200 as V
 from direct_visual_lidar_calibration_b200 import bfgs
+from direct_visual_lidar_calibration_b200.calibration import outer_step_delta
 
 
 def make_T(rotvec, t):
@@ -74,6 +75,7 @@ def test_invalid_start_is_reported_not_hidden():
     T0 = make_T([0, 0, 0], [0, 0, 0])
     T, r = bfgs.minimize_se3(lambda x: (False, 0.0, np.zeros(7)), T0)
     assert r["termination"] == "failure" and np.allclose(T, T0)
+    assert r["evaluations"] == 1 and r["iterations"] == 0  # the start pose was evaluated once
 
 
 def test_objective_invalid_in_a_region():
@@ -125,6 +127,69 @@ def test_registration_type_enum_and_params():
     d = bfgs.default_bfgs_params()
     assert d.max_num_iterations == 50 and d.function_tolerance == 1e-6 and d.gradient_tolerance == 1e-10 and d.parameter_tolerance == 1e-8
     assert d.max_translation_from_init == 0.2 and abs(d.max_rotation_from_init - np.deg2rad(2.0)) < 1e-15
+
+
+def _steps_at_the_threshold(O, T0, w, v, component, thresh, ulps=4):
+    """Outer-loop results new_T(s) = T0 * Expmap(s w, s v) whose oracle step (delta_t if component == 0, delta_r if 1)
+    straddles `thresh`: bisection over s down to adjacent doubles, then the first s that reaches the threshold and
+    `ulps` doubles either side of it."""
+    def new_T(s):
+        return O.isometry_mul(T0, O.se3_expmap(np.concatenate([s * np.asarray(w), s * np.asarray(v)])))
+
+    lo, hi = 0.0, 1.0
+    assert O.outer_step_delta(T0, new_T(lo))[component] < thresh <= O.outer_step_delta(T0, new_T(hi))[component]
+    while np.nextafter(lo, hi) != hi:
+        mid = 0.5 * (lo + hi)
+        if mid in (lo, hi):
+            mid = np.nextafter(lo, hi)
+        if O.outer_step_delta(T0, new_T(mid))[component] < thresh:
+            lo = mid
+        else:
+            hi = mid
+    ss = [hi]
+    for _ in range(ulps):
+        ss = [np.nextafter(ss[0], -np.inf)] + ss + [np.nextafter(ss[-1], np.inf)]
+    return [new_T(s) for s in ss]
+
+
+@pytest.mark.parametrize("component", ["translation", "rotation"])
+def test_bfgs_outer_loop_stops_on_the_reference_rule(oracle, component):
+    """The NID_BFGS outer loop (visual_camera_calibration.cpp:35-68) stops when delta = new_T^-1 * T, as isometries, has
+    |translation| < delta_trans_thresh and AngleAxisd angle < delta_rot_thresh.  The inner solve is replaced by a stub
+    returning chosen poses placed at each threshold to the ulp, so the decision and the outer-iteration count must be
+    the oracle rule's bit for bit: a general 4x4 inverse, np.linalg.norm or arccos of the trace would stop on a
+    different outer iteration for some of these poses."""
+    params = V.VisualCameraCalibrationParams()
+    params.registration_type = V.RegistrationType.NID_BFGS
+    T0 = make_T([0.3, -0.2, 0.5], [1.0, 2.0, -0.5])
+    if component == "translation":  # rotation of the step well inside its threshold, translation at 0.1 m
+        w, v, k, thresh = [0.01, -0.02, 0.015], [0.6, -0.5, 0.7], 0, params.delta_trans_thresh
+    else:  # translation well inside, rotation at 0.5 deg
+        w, v, k, thresh = [0.6, -0.5, 0.7], [0.8, 0.5, -0.6], 1, params.delta_rot_thresh
+    decisions, general_rule_differs = [], False
+    for new_T in _steps_at_the_threshold(oracle, T0, w, v, k, thresh):
+        dt, dr = oracle.outer_step_delta(T0, new_T)
+        assert outer_step_delta(T0, new_T) == (dt, dr)
+        stop = dt < params.delta_trans_thresh and dr < params.delta_rot_thresh
+        decisions.append(stop)
+        # the general-matrix rule this loop must not use: it decides at least one of these poses differently
+        d = np.linalg.inv(new_T) @ T0
+        g_dt, g_dr = np.linalg.norm(d[:3, 3]), np.arccos(np.clip(0.5 * (np.trace(d[:3, :3]) - 1.0), -1.0, 1.0))
+        general_rule_differs |= (g_dt < params.delta_trans_thresh and g_dr < params.delta_rot_thresh) != stop
+        # the stub's second solve returns its start pose: delta 0, the loop stops there at the latest
+        calls = []
+
+        def stub(T, _new_T=new_T):
+            calls.append(np.array(T))
+            return (_new_T if len(calls) == 1 else np.array(T)), {"evaluations": 1}
+
+        calib = V.VisualCameraCalibration(None, [], params)
+        calib.estimate_pose_bfgs = stub
+        T = calib.calibrate(T0)
+        assert calib.stats["outer_iterations"] == (1 if stop else 2), (component, dt, dr)
+        assert np.array_equal(T, new_T) and np.array_equal(calls[0], T0)
+    assert True in decisions and False in decisions  # the poses straddle the threshold
+    assert general_rule_differs  # so the stub loop above fails on the old rule for this component
 
 
 BFGS_WORKER = r"""
