@@ -115,6 +115,14 @@ class ScanDesc(C.Structure):
     ]
 
 
+class Frame(C.Structure):
+    """vlcal_frame: one compressed container frame (zstd or LZ4 frame format) and where its output goes."""
+    _fields_ = [
+        ("src_offset", C.c_int64), ("src_size", C.c_int64), ("dst_offset", C.c_int64), ("dst_size", C.c_int64), ("codec", C.c_int32),
+        ("has_crc32", C.c_int32), ("crc32", C.c_uint32), ("reserved", C.c_int32),
+    ]
+
+
 class SearchSet(C.Structure):
     """vlcal_search_set: pose i = (ib * n_left + il) * n_offset + io is [R | R (center[ib] + offset[io])], R = left[il] base[ib]."""
     _fields_ = [
@@ -234,6 +242,7 @@ def load_library():
     L.vlcal_lidar_fov_candidates.argtypes = [C.c_int, vp, C.c_int64, vp, i64p, ip, dp]
     L.vlcal_min_bearing_cosine.argtypes = [C.c_int, vp, C.c_int64, dp]
     L.vlcal_bag_integrate.argtypes = [C.c_int, vp, C.c_int64, C.POINTER(ScanDesc), C.c_int64, C.c_double, C.c_double, vp, i64p, i64p, dp]
+    L.vlcal_decode_frames.argtypes = [C.c_int, vp, C.c_int64, C.POINTER(Frame), C.c_int, vp, C.c_int64, C.POINTER(C.c_int32), dp]
     _lib = L
     return L
 

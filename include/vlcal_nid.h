@@ -794,6 +794,50 @@ int vlcal_bag_integrate(
   int64_t* out_of_range_points,
   double* stage_ms_out);
 
+/* ---- compressed bag chunks (DESIGN §4f) ---------------------------------------------------------------------------
+ * A batch of independent frames decoded on the GPU: MCAP chunks (zstd, lz4), ROS 1 lz4 chunks, rosbag2 zstd messages.
+ * A frame's src range holds one or more concatenated frames of its codec, skippable frames among them:
+ *   VLCAL_CODEC_ZSTD        zstd (RFC 8878) without dictionaries; the content checksum is verified when present.
+ *   VLCAL_CODEC_LZ4_FRAME   the LZ4 frame format (magic 0x184D2204), linked or independent blocks, uncompressed blocks;
+ *                           the header, block and content checksums are verified when present.
+ * It must decode to exactly dst_size bytes, written to dst[dst_offset, dst_offset + dst_size).  has_crc32: crc32 is the
+ * CRC-32 (zlib polynomial) of those bytes and is verified (MCAP's uncompressed_crc when it is not 0). */
+#define VLCAL_CODEC_ZSTD 1
+#define VLCAL_CODEC_LZ4_FRAME 2
+typedef struct {
+  int64_t src_offset;
+  int64_t src_size;
+  int64_t dst_offset;
+  int64_t dst_size;
+  int32_t codec;
+  int32_t has_crc32;
+  uint32_t crc32;
+  int32_t reserved;
+} vlcal_frame;
+
+/* per-frame status_out */
+#define VLCAL_FRAME_OK 0
+#define VLCAL_FRAME_CORRUPT 1          /* malformed, truncated, or a match reaching before the start of its output */
+#define VLCAL_FRAME_CHECKSUM 2         /* a checksum of the format, or crc32, does not match */
+#define VLCAL_FRAME_SIZE 3             /* the frame decodes to a size other than dst_size */
+#define VLCAL_FRAME_UNSUPPORTED 4      /* a zstd or LZ4 dictionary id, the legacy LZ4 format, a window above 2 GiB */
+
+/* Decodes frames[0, n_frames) from host src[0, src_bytes) into host dst[0, dst_bytes); status_out[i] is frame i's
+ * status.  The dst bytes of a frame whose status is not 0 are unspecified; bytes of dst outside every frame's range are
+ * not touched.  Checked on the host before any GPU work (VLCAL_ERR_INVALID_ARGUMENT): a known codec, has_crc32 0 or 1,
+ * every range inside its buffer, no two non-empty dst ranges overlapping.  Malformed frame data never reads or writes
+ * outside the frame's own ranges.  ms_out (optional, 3 doubles): copy in, kernel, copy out, between CUDA events. */
+int vlcal_decode_frames(
+  int device,
+  const uint8_t* src,
+  int64_t src_bytes,
+  const vlcal_frame* frames,
+  int n_frames,
+  uint8_t* dst,
+  int64_t dst_bytes,
+  int32_t* status_out,
+  double* ms_out);
+
 #ifdef __cplusplus
 }
 #endif
