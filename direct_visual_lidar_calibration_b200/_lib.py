@@ -254,7 +254,7 @@ def check(rc: int):
 
 
 def set_solver_mode(mode: int):
-    """0 auto (persistent kernel where possible), 1 host loop, 2 device-resident loop, 3 persistent kernel (see include/vlcal_nid.h)."""
+    """0 auto (persistent kernel where possible), 1 host loop, 3 persistent kernel (see include/vlcal_nid.h); any other mode raises VlcalError."""
     check(load_library().vlcal_nid_set_solver_mode(int(mode)))
 
 

@@ -22,7 +22,7 @@ double now_ms() {
 }
 
 vlcal_p2p* g_default_p2p = nullptr;  // vlcal_nid_p2p_set_default
-int g_solver_mode = 0;                // vlcal_nid_set_solver_mode: 0 auto, 1 host loop, 2 device-resident loop
+int g_solver_mode = 0;                // vlcal_nid_set_solver_mode: 0 auto, 1 host loop, 3 persistent kernel
 thread_local bool g_record_solve_trace = false;  // vlcal_nid_debug_record_solve_trace
 thread_local std::vector<double> g_solve_trace;  // [k][7]: solve_trace_push
 
@@ -91,108 +91,6 @@ struct PoseObjective {
   }
 };
 
-// Device-resident inner solve: the Nelder-Mead state machine advances inside the finalizing block of each launch
-// (nid_kernels.cuh: nm_device_advance), the host only enqueues launches in chunks and replays the best-cost callback
-// from the evaluation trace afterwards (same order as the reference, delivered up to one chunk late).
-constexpr int DEVICE_LOOP_CHUNK = 24;
-
-struct PoolPtr {
-  void* p = nullptr;
-  int device = 0;
-  bool pinned = false;
-  ~PoolPtr() {
-    if (pinned) MemPool::instance().pinned_free(p);
-    else MemPool::instance().device_free(device, p);
-  }
-};
-
-int run_inner_solve_device(
-  vlcal_nid_ctx* ctx, const vlcal_calib_params* params, const double init_T[16], vlcal_pose_callback callback, void* user, double T_out[16], vlcal_nm_result* nm_result) {
-  VL_CUDA(cudaSetDevice(ctx->device));
-  NmParams nm;  // visual_camera_calibration.cpp:122-125
-  nm.init_step = params->nelder_mead_init_step;
-  nm.convergence_var_thresh = params->nelder_mead_convergence_criteria;
-  nm.max_iterations = params->max_inner_iterations;
-
-  PoolPtr h_state, d_state, d_trace, h_trace;
-  h_state.pinned = true, h_trace.pinned = true;
-  d_state.device = d_trace.device = ctx->device;
-  const int trace_cap = 16 + std::max(0, params->max_inner_iterations) * (NM_MAX_N + 1);
-  const size_t trace_bytes = sizeof(double) * (NM_MAX_N + 1) * static_cast<size_t>(trace_cap);
-  VL_CUDA(MemPool::instance().pinned_alloc(sizeof(NmDevice), &h_state.p));
-  VL_CUDA(MemPool::instance().device_alloc(ctx->device, sizeof(NmDevice), &d_state.p));
-  VL_CUDA(MemPool::instance().device_alloc(ctx->device, trace_bytes, &d_trace.p));
-  VL_CUDA(MemPool::instance().pinned_alloc(trace_bytes, &h_trace.p));
-
-  NmDevice* h = static_cast<NmDevice*>(h_state.p);
-  std::memset(static_cast<void*>(h), 0, sizeof(NmDevice));
-  const double x0[6] = {0, 0, 0, 0, 0, 0};
-  h->nm.begin(6, nm, x0);  // :126 optimize(f, Zero)
-  std::memcpy(h->init_T, init_T, sizeof(h->init_T));
-  for (int k = 0; k < h->nm.n_cand; k++) nm_pose_of_candidate(h->nm.cand[k], h->init_T, h, k);
-  h->n_poses = h->nm.n_cand;
-  h->trace_cap = trace_cap;
-  h->trace_count = 0;
-  h->trace = static_cast<double*>(d_trace.p);
-  VL_CUDA(cudaMemcpyAsync(d_state.p, h, sizeof(NmDevice), cudaMemcpyHostToDevice, ctx->stream));
-
-  double best_cost = DBL_MAX;  // :101
-  int trace_seen = 0;
-  unsigned long long steps_seen = 0;
-  int computed_seen = 0;
-  const double* trace = static_cast<const double*>(h_trace.p);
-  for (;;) {
-    int rc = nid_enqueue_device_steps(ctx, static_cast<NmDevice*>(d_state.p), DEVICE_LOOP_CHUNK);
-    if (rc != VLCAL_OK) return rc;
-    VL_CUDA(cudaMemcpyAsync(h, d_state.p, sizeof(NmDevice), cudaMemcpyDeviceToHost, ctx->stream));
-    VL_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (ctx->p2p && ctx->p2p->h_error && *ctx->p2p->h_error) {
-      set_last_error("peer exchange timed out: a rank died or the ranks are not evaluating in lockstep");
-      return VLCAL_ERR_CUDA;
-    }
-    rc = nid_account_device_steps(ctx, DEVICE_LOOP_CHUNK, static_cast<int>(h->steps_done - steps_seen), h->nm.num_evaluations_computed - computed_seen);
-    if (rc != VLCAL_OK) return rc;
-    steps_seen = h->steps_done;
-    computed_seen = h->nm.num_evaluations_computed;
-    const int count = std::min(h->trace_count, trace_cap);
-    if (count > trace_seen) {  // replay the objective's side effects in the reference's order (:112-116)
-      const size_t stride = NM_MAX_N + 1;
-      VL_CUDA(cudaMemcpy(const_cast<double*>(trace) + stride * trace_seen, static_cast<double*>(d_trace.p) + stride * trace_seen, sizeof(double) * stride * (count - trace_seen), cudaMemcpyDeviceToHost));
-      for (int k = trace_seen; k < count; k++) {
-        const double* e = trace + stride * k;
-        const double y = e[NM_MAX_N];
-        solve_trace_push(e, y);
-        if (y < best_cost) {
-          best_cost = y;
-          if (callback) {
-            double E[16], T[16];
-            host::se3_expmap_gtsam(e, E);
-            host::isometry_mul(init_T, E, T);
-            callback(T, y, user);
-          }
-        }
-      }
-      trace_seen = count;
-    }
-    if (h->nm.phase == 3) break;
-    if (h->steps_done == steps_seen && h->n_poses == 0) break;  // defensive: nothing left to do
-  }
-  double E[16];
-  host::se3_expmap_gtsam(h->nm.result_x, E);
-  host::isometry_mul(init_T, E, T_out);  // :129
-  if (nm_result) {
-    std::memset(nm_result, 0, sizeof(*nm_result));
-    nm_result->converged = h->nm.converged;
-    nm_result->num_iterations = h->nm.num_iterations;
-    for (int d = 0; d < 6; d++) nm_result->x[d] = h->nm.result_x[d];
-    nm_result->y = h->nm.result_y;
-    nm_result->num_evaluations = h->nm.num_evaluations;
-    nm_result->num_batches = h->nm.num_batches;
-    nm_result->num_evaluations_computed = h->nm.num_evaluations_computed;
-  }
-  return VLCAL_OK;
-}
-
 int run_inner_solve(
   vlcal_nid_ctx* const* ctxs, int n_ctxs, const vlcal_calib_params* params, const double init_T[16], vlcal_pose_callback callback, vlcal_allreduce_fn allreduce, void* user,
   double T_out[16], vlcal_nm_result* nm_result) {
@@ -211,18 +109,6 @@ int run_inner_solve(
   }
   if (pk_ok && (g_solver_mode == 0 || g_solver_mode == 3)) {
     return pk_solve(ctxs, n_ctxs, params, init_T, callback, user, T_out, nm_result);
-  }
-  // one bag on this GPU, scores either local or summed in-kernel over the peer exchange: the round-1 device-resident loop
-  // (one launch per batch, machine stepped by the finalizing block).  (Several local bags, or a host-side all-reduce
-  // callback, need the host between batches.)
-  const bool device_ok = n_ctxs == 1 && ctxs[0]->mode == VLCAL_NID_MODE_HISTOGRAM && ctxs[0]->max_poses >= NID_MAX_POSES && (allreduce == nullptr || ctx_exchange_is_fused(ctxs[0])) &&
-                         params->max_inner_iterations >= 0;
-  if (g_solver_mode == 2 && !device_ok) {
-    set_last_error("device-resident solver loop requested but this solve needs the host between batches (several local bags / host all-reduce / bins too large)");
-    return VLCAL_ERR_UNSUPPORTED;
-  }
-  if (device_ok && g_solver_mode == 2) {
-    return run_inner_solve_device(ctxs[0], params, init_T, callback, user, T_out, nm_result);
   }
   if (n_ctxs > 1 && px_fused) {
     // the round-1 kernels exchange one bag per rank; with several local bags only the persistent kernel sums in-kernel
@@ -394,8 +280,12 @@ int vlcal_nid_debug_last_solve_trace(int capacity, double* rows_out, int* n_out)
 }
 
 int vlcal_nid_set_solver_mode(int mode) {
+  if (mode == 2) {
+    set_last_error("solver mode 2: the round-1 device-resident loop was removed; use 0 (auto), 1 (host loop) or 3 (persistent kernel)");
+    return VLCAL_ERR_INVALID_ARGUMENT;
+  }
   if (mode < 0 || mode > 3) {
-    set_last_error("solver mode must be 0 (auto), 1 (host loop), 2 (device-resident loop) or 3 (persistent kernel)");
+    set_last_error("solver mode must be 0 (auto), 1 (host loop) or 3 (persistent kernel)");
     return VLCAL_ERR_INVALID_ARGUMENT;
   }
   g_solver_mode = mode;

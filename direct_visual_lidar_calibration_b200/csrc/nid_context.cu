@@ -281,27 +281,23 @@ int upload_image(int device, const uint8_t* image, int width, int height, int ro
 using NidKernel = void (*)(const NidArgs);
 
 // kind: 0 = fp32 filter + exact recheck (float4 layout only; 4 points/thread), 1 = exact fp64, 2 = verify (debug),
-//       3 = fp32 filter with 2 points/thread (A/B measurement); devloop: device-resident solver-loop variant of 0 / 1
+//       3 = fp32 filter with 2 points/thread (A/B measurement)
 template <int MODEL>
-static NidKernel pick_layout(bool f32, int kind, bool devloop) {
-  if (devloop) {
-    if (f32 && (kind == 0 || kind == 3)) return nid_hist_filter_kernel<MODEL, true, 4, true>;
-    return f32 ? nid_hist_exact_kernel<MODEL, true, true> : nid_hist_exact_kernel<MODEL, false, true>;
-  }
-  if (f32 && kind == 0) return nid_hist_filter_kernel<MODEL, true, 4, false>;
-  if (f32 && kind == 3) return nid_hist_filter_kernel<MODEL, true, 2, false>;
+static NidKernel pick_layout(bool f32, int kind) {
+  if (f32 && kind == 0) return nid_hist_filter_kernel<MODEL, true, 4>;
+  if (f32 && kind == 3) return nid_hist_filter_kernel<MODEL, true, 2>;
   if (f32 && kind == 2) return nid_filter_verify_kernel<MODEL, true>;
-  return f32 ? nid_hist_exact_kernel<MODEL, true, false> : nid_hist_exact_kernel<MODEL, false, false>;
+  return f32 ? nid_hist_exact_kernel<MODEL, true> : nid_hist_exact_kernel<MODEL, false>;
 }
 
-static NidKernel pick_kernel(int model, bool f32, int kind, bool devloop = false) {
+static NidKernel pick_kernel(int model, bool f32, int kind) {
   switch (model) {
-    case CAM_PLUMB_BOB: return pick_layout<CAM_PLUMB_BOB>(f32, kind, devloop);
-    case CAM_FISHEYE: return pick_layout<CAM_FISHEYE>(f32, kind, devloop);
-    case CAM_ATAN: return pick_layout<CAM_ATAN>(f32, kind, devloop);
-    case CAM_OMNIDIR: return pick_layout<CAM_OMNIDIR>(f32, kind, devloop);
-    case CAM_EQUIRECTANGULAR: return pick_layout<CAM_EQUIRECTANGULAR>(f32, kind, devloop);
-    case CAM_RATIONAL_POLYNOMIAL: return pick_layout<CAM_RATIONAL_POLYNOMIAL>(f32, kind, devloop);
+    case CAM_PLUMB_BOB: return pick_layout<CAM_PLUMB_BOB>(f32, kind);
+    case CAM_FISHEYE: return pick_layout<CAM_FISHEYE>(f32, kind);
+    case CAM_ATAN: return pick_layout<CAM_ATAN>(f32, kind);
+    case CAM_OMNIDIR: return pick_layout<CAM_OMNIDIR>(f32, kind);
+    case CAM_EQUIRECTANGULAR: return pick_layout<CAM_EQUIRECTANGULAR>(f32, kind);
+    case CAM_RATIONAL_POLYNOMIAL: return pick_layout<CAM_RATIONAL_POLYNOMIAL>(f32, kind);
     default: return nullptr;
   }
 }
@@ -507,7 +503,7 @@ static void fill_common_args(vlcal_nid_ctx* ctx, NidArgs& a) {
   a.counter = ctx->d_counter;
 }
 
-static NidKernel select_kernel(vlcal_nid_ctx* ctx, bool devloop = false) {
+static NidKernel select_kernel(vlcal_nid_ctx* ctx) {
   // the fp32 filter needs the float4 layout, a camera/FoV it has bounds for, and 32-bit point indices
   const bool use_filter = ctx->variant != 1 && ctx->cloud->f32 && ctx->fast.enabled && ctx->cloud->n < 0x7fffffffLL;
   // points per lane and tile (tools/kernel_scaling.py measures the choice):
@@ -519,15 +515,15 @@ static NidKernel select_kernel(vlcal_nid_ctx* ctx, bool devloop = false) {
   const long long points_per_warp = ctx->cloud->n / (static_cast<long long>(ctx->num_sms) * 2 * (NID_THREADS / 32));
   const bool four = !heavy && points_per_warp >= 96 && points_per_warp <= 1100;
   const int filter_kind = ctx->variant == 2 ? 3 : (ctx->variant == 3 ? 0 : (four ? 0 : 3));
-  return pick_kernel(ctx->cam.model, ctx->cloud->f32, use_filter ? filter_kind : 1, devloop);
+  return pick_kernel(ctx->cam.model, ctx->cloud->f32, use_filter ? filter_kind : 1);
 }
 
 constexpr int PROFILE_STRIDE = 4;
 
-static int launch_one(vlcal_nid_ctx* ctx, NidKernel kernel, NidArgs& a, int geometry_poses, int profile_poses) {
+static int launch_one(vlcal_nid_ctx* ctx, NidKernel kernel, NidArgs& a) {
   LaunchGeom g{1, 0, 1, 0};
   {
-    const int rc = launch_geometry(ctx->device, kernel, geometry_poses, a.nb, a.bins, &g);
+    const int rc = launch_geometry(ctx->device, kernel, a.n_poses, a.nb, a.bins, &g);
     if (rc != VLCAL_OK) return rc;
   }
   a.copies = g.copies;
@@ -545,7 +541,7 @@ static int launch_one(vlcal_nid_ctx* ctx, NidKernel kernel, NidArgs& a, int geom
       ctx->events.push_back(e);
     }
     ev = &ctx->events[ctx->events_used++];
-    ev->poses = profile_poses;
+    ev->poses = a.n_poses;
     VL_CUDA(cudaEventRecord(ev->start, ctx->stream));
   }
   kernel<<<grid, NID_THREADS, g.smem, ctx->stream>>>(a);
@@ -587,7 +583,7 @@ int nid_evaluate_async(vlcal_nid_ctx* ctx, const double* T_colmajor, int n_poses
     a.done_flag = last_chunk ? ctx->h_flag : nullptr;
     a.done_seq = ctx->seq + 1;
     a.hist_out = want_hist ? ctx->d_hist_out + static_cast<size_t>(p0) * nb : nullptr;
-    const int rc = launch_one(ctx, kernel, a, pc, pc);
+    const int rc = launch_one(ctx, kernel, a);
     if (rc != VLCAL_OK) return rc;
     ctx->launches++;
     ctx->passes++;
@@ -597,64 +593,6 @@ int nid_evaluate_async(vlcal_nid_ctx* ctx, const double* T_colmajor, int n_poses
   ctx->in_flight = true;
   ctx->in_flight_hist = want_hist;
   ctx->in_flight_poses = n_poses;
-  return VLCAL_OK;
-}
-
-int nid_enqueue_device_steps(vlcal_nid_ctx* ctx, NmDevice* d_nm, int count) {
-  if (ctx->in_flight) {
-    set_last_error("an evaluation is in flight on this context");
-    return VLCAL_ERR_BUSY;
-  }
-  if (ctx->mode != VLCAL_NID_MODE_HISTOGRAM) {
-    set_last_error("device-resident solver loop needs a histogram-mode context");
-    return VLCAL_ERR_INVALID_ARGUMENT;
-  }
-  VL_CUDA(cudaSetDevice(ctx->device));
-  {
-    const int rc = ensure_outputs(ctx, NID_MAX_POSES, false);
-    if (rc != VLCAL_OK) return rc;
-  }
-  if (ctx->max_poses < NID_MAX_POSES) {
-    set_last_error("device-resident solver loop needs room for 8 poses per launch (bins too large)");
-    return VLCAL_ERR_UNSUPPORTED;
-  }
-  NidKernel kernel = select_kernel(ctx, /*devloop=*/true);
-  NidArgs a;
-  fill_common_args(ctx, a);
-  a.nm = d_nm;
-  a.n_poses = 0;
-  a.nid_out = ctx->d_nid;
-  for (int k = 0; k < count; k++) {
-    const int rc = launch_one(ctx, kernel, a, NID_MAX_POSES, 0);
-    if (rc != VLCAL_OK) return rc;
-  }
-  return VLCAL_OK;
-}
-
-int nid_account_device_steps(vlcal_nid_ctx* ctx, int enqueued, int worked, int poses) {
-  // sampled events of this enqueue: keep those of launches that did work, drop the ones that found the solver finished
-  if (ctx->profiling) {
-    const int64_t first_launch = ctx->launch_counter - enqueued;  // index of the first launch of this enqueue
-    int sampled = 0;
-    for (int k = 0; k < enqueued; k++)
-      if (((first_launch + k) % PROFILE_STRIDE) == 0) sampled++;
-    const size_t first = ctx->events_used - static_cast<size_t>(sampled);
-    int e = 0;
-    for (int k = 0; k < enqueued; k++) {
-      if (((first_launch + k) % PROFILE_STRIDE) != 0) continue;
-      if (k < worked) {
-        float ms = 0.f;
-        VL_CUDA(cudaEventElapsedTime(&ms, ctx->events[first + e].start, ctx->events[first + e].stop));
-        ctx->kernel_ms_accum += ms;
-        ctx->timed_launches++;
-      }
-      e++;
-    }
-    ctx->events_used = first;
-  }
-  ctx->launches += worked;
-  ctx->passes += worked;
-  ctx->poses_total += poses;
   return VLCAL_OK;
 }
 

@@ -152,11 +152,6 @@ int nid_ctx_create(
   int device, int mode, const CameraParams& cam, std::shared_ptr<DeviceImage> image, std::shared_ptr<DeviceCloud> cloud, int bins, double max_fov, vlcal_nid_ctx** out);
 int nid_evaluate_async(vlcal_nid_ctx* ctx, const double* T_colmajor, int n_poses, bool want_hist);
 int nid_wait(vlcal_nid_ctx* ctx, double* nid_out, int32_t* hist_out);
-struct NmDevice;
-// device-resident solver loop: enqueue `count` launches that read their poses from / advance `d_nm`; no waiting
-int nid_enqueue_device_steps(vlcal_nid_ctx* ctx, NmDevice* d_nm, int count);
-// after the stream was synchronised: account the first `worked` launches of the last enqueue in the profile
-int nid_account_device_steps(vlcal_nid_ctx* ctx, int enqueued, int worked, int poses);
 
 // persistent cooperative kernel (nid_persistent.cu): can these contexts (bags of one camera on one device) run on it?
 bool pk_supported(vlcal_nid_ctx* const* ctxs, int n_ctxs);

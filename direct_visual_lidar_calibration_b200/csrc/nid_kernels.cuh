@@ -11,8 +11,8 @@
 //   per block  : P x bins x bins int32 histogram copies in shared memory, merged into the global accumulator with
 //                one red.global.add per non-zero bin
 //   last block : marginals (row/column sums), the three entropies, MI and NID for every pose; optionally the sum over
-//                ranks (NVLink peer-memory exchange) and the next Nelder-Mead batch (device-resident loop); results
-//                published to mapped host memory; accumulators zeroed again so the next launch needs no memset.
+//                ranks (NVLink peer-memory exchange); results published to mapped host memory; accumulators zeroed
+//                again so the next launch needs no memset.
 // Algorithmic traffic: 16 B/point + W*H B of image per pass regardless of P (DESIGN.md section 5); the active bound is
 // instruction issue (108 warp-instructions per point-pose) and, for Nelder-Mead sized batches, the serial tail.
 #pragma once
@@ -20,8 +20,6 @@
 #include <cstdint>
 
 #include "camera_models.cuh"
-#include "nm_machine.cuh"
-#include "se3_math.cuh"
 
 namespace vlcal {
 
@@ -42,24 +40,6 @@ struct P2PMailbox {
   unsigned long long ll[P2P_MAX_RANKS][2][8][2];  // [sender][slot][pose][lo, hi]
 };
 
-// ---- device-resident Nelder-Mead loop ---------------------------------------------------------------------
-// With NidArgs::nm set, a launch takes its candidate poses from this block of device memory instead of from its kernel
-// parameters, and the finalizing block -- once the scores of the batch are known -- advances the Nelder-Mead state
-// machine (nm_machine.cuh) and writes the NEXT batch of poses T = init_T * Expmap(x) back into it.  The host can then
-// enqueue many launches back to back without waiting for any of them: the per-iteration host round trip (launch
-// latency + PCIe + wake-up) disappears from the critical path.  Launches enqueued after
-// the solver finished see n_poses == 0 and exit at once.
-struct NmDevice {
-  NmMachine nm;
-  double init_T[16];                    // column-major start pose (visual_camera_calibration.cpp:104)
-  double pose[NID_MAX_POSES][12];       // pending batch: row-major 3x4 [R|t]
-  float pose32[NID_MAX_POSES][16];      // fp32 filter copy (R, t, max|t|)
-  int n_poses;                          // poses of the pending batch; 0 once finished
-  int trace_cap, trace_count;           // reference-order evaluations (x[6], y) for callback replay on the host
-  double* trace;
-  unsigned long long steps_done;
-};
-
 struct NidArgs {
   const void* points;        // float4[n] (x,y,z,intensity) or double4[n]
   const uint8_t* bin_image;  // H x W image bins: clamp(int(u8/255.0*bins), 0, bins-1)  (:43,:46)
@@ -78,9 +58,8 @@ struct NidArgs {
   P2PMailbox* peer_box[P2P_MAX_RANKS];  // peer_box[r]: rank r's mailbox as mapped in this process (self included)
   int p2p_world, p2p_rank;         // p2p_world <= 1: no exchange
   int* p2p_error;                  // mapped host word, set to 1 if a peer never answered
-  unsigned long long* p2p_counter; // device word: number of exchanges done (kept on the device so that it only advances
-                                   // when an exchange really happens -- launches that exit early do not consume a slot)
-  NmDevice* nm;                    // device-resident solver loop (nullptr: poses come from the kernel parameters)
+  unsigned long long* p2p_counter; // device word: number of exchanges done (advanced by the finalizing block of every
+                                   // exchanging launch, so all ranks number their exchanges alike)
   unsigned long long* timeline;    // optional [16] mapped host words: globaltimer stamps of the launch (vlcal_nid_debug_timeline)
   int* ghist;                 // [NID_MAX_POSES][nb] global accumulators, zero on entry, zero on exit
   unsigned int* counter;      // block ticket, zero on entry, zero on exit
@@ -90,23 +69,6 @@ struct NidArgs {
   unsigned long long done_seq;
   int* hist_out;              // optional [n_poses][nb], index = image_bin + lidar_bin*bins
 };
-
-// where a launch reads its poses from: kernel parameters (constant bank) or, in the device-resident loop, NmDevice
-template <bool DEVLOOP>
-__device__ __forceinline__ int n_poses_of(const NidArgs& a) {
-  if constexpr (DEVLOOP) return a.nm->n_poses;
-  else return a.n_poses;
-}
-template <bool DEVLOOP>
-__device__ __forceinline__ const double* pose_of(const NidArgs& a, int p) {
-  if constexpr (DEVLOOP) return a.nm->pose[p];
-  else return a.pose[p];
-}
-template <bool DEVLOOP>
-__device__ __forceinline__ const float* pose32_of(const NidArgs& a, int p) {
-  if constexpr (DEVLOOP) return a.nm->pose32[p];
-  else return a.pose32[p];
-}
 
 // ---- exact decision for one (point, pose): pixel index iy*W+ix (>= 0), or -1 if the reference skips the point
 template <int MODEL>
@@ -294,64 +256,6 @@ static __device__ void nid_peer_allreduce(const NidArgs& a, int n_poses) {
   __syncthreads();
 }
 
-// T = init_T * Expmap(x) for one candidate of the pending batch (visual_camera_calibration.cpp:104) -> pose / pose32 slot k
-VL_HD void nm_pose_of_candidate(const double* cand_vertex, const double* init_T, NmDevice* out, int k) {
-  double E[16], T[16];
-  se3_expmap_gtsam_hd(cand_vertex + 1, E);
-  isometry_mul_hd(init_T, E, T);
-  double tmax = 0.0;
-  for (int r = 0; r < 3; r++) {
-    for (int c = 0; c < 4; c++) out->pose[k][4 * r + c] = T[r + 4 * c];
-    for (int c = 0; c < 3; c++) out->pose32[k][3 * r + c] = static_cast<float>(T[r + 4 * c]);
-    out->pose32[k][9 + r] = static_cast<float>(T[r + 12]);
-    tmax = fmax(tmax, fabs(T[r + 12]));
-  }
-  out->pose32[k][12] = nextafterf(static_cast<float>(tmax), INFINITY);  // max|t| rounded up (fp32 filter bound)
-  out->pose32[k][13] = out->pose32[k][14] = out->pose32[k][15] = 0.f;
-}
-
-// device-resident solver loop: consume the scores of the batch, advance the state machine, emit the next poses.
-// The machine is staged in shared memory: stepping it in place in HBM would be hundreds of dependent L2 round trips.
-static __device__ void nm_device_advance(const NidArgs& a) {
-  static_assert(sizeof(NmMachine) % 8 == 0, "NmMachine is copied as 8-byte words");
-  __shared__ NmMachine s_nm;
-  __shared__ double s_init_T[16];
-  NmDevice* nm = a.nm;
-  {
-    const unsigned long long* src = reinterpret_cast<const unsigned long long*>(&nm->nm);
-    unsigned long long* dst = reinterpret_cast<unsigned long long*>(&s_nm);
-    for (int i = threadIdx.x; i < static_cast<int>(sizeof(NmMachine) / 8); i += blockDim.x) dst[i] = src[i];
-    if (threadIdx.x < 16) s_init_T[threadIdx.x] = nm->init_T[threadIdx.x];
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    s_nm.step(a.nid_out);
-    const int n = s_nm.n;
-    int count = nm->trace_count;
-    for (int k = 0; k < s_nm.n_obs; k++) {  // reference-order evaluations, replayed by the host for params.callback
-      if (count < nm->trace_cap) {
-        double* e = nm->trace + static_cast<size_t>(count) * (NM_MAX_N + 1);
-        for (int d = 0; d < n; d++) e[d] = s_nm.obs_x[k][d];
-        e[NM_MAX_N] = s_nm.obs_y[k];
-      }
-      count++;
-    }
-    nm->trace_count = count;
-    nm->steps_done++;
-  }
-  __syncthreads();
-  {
-    const unsigned long long* src = reinterpret_cast<const unsigned long long*>(&s_nm);
-    unsigned long long* dst = reinterpret_cast<unsigned long long*>(&nm->nm);
-    for (int i = threadIdx.x; i < static_cast<int>(sizeof(NmMachine) / 8); i += blockDim.x) dst[i] = src[i];
-  }
-  const int n_next = s_nm.n_cand;  // 0 when finished
-  if (threadIdx.x < n_next) nm_pose_of_candidate(s_nm.cand[threadIdx.x], s_init_T, nm, threadIdx.x);
-  __syncthreads();
-  if (threadIdx.x == 0) nm->n_poses = n_next;
-}
-
-template <bool DEVLOOP>
 static __device__ void nid_finalize(const NidArgs& a, int n_poses, int* smem_i) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, n_warps = blockDim.x >> 5;
   __shared__ int s_cnt[NID_THREADS / 32];  // per-warp partial inlier counts
@@ -465,7 +369,6 @@ static __device__ void nid_finalize(const NidArgs& a, int n_poses, int* smem_i) 
     __syncthreads();
   }
   if (a.p2p_world > 1) nid_peer_allreduce(a, n_poses);
-  if constexpr (DEVLOOP) nm_device_advance(a);
   stamp(a, 4);
   if (threadIdx.x == 0) {
     *a.counter = 0u;
@@ -478,7 +381,6 @@ static __device__ void nid_finalize(const NidArgs& a, int n_poses, int* smem_i) 
 }
 
 // block epilogue shared by the histogram kernels: merge copies -> global accumulators -> last block finalizes
-template <bool DEVLOOP>
 __device__ __forceinline__ void nid_block_epilogue(const NidArgs& a, int n_poses, int* smem_hist, bool* s_is_last) {
   const int per_copy = n_poses * a.nb;
   const unsigned long long t_main = a.timeline ? global_ns() : 0ull;
@@ -503,17 +405,14 @@ __device__ __forceinline__ void nid_block_epilogue(const NidArgs& a, int n_poses
     a.timeline[3] = global_ns();
   }
   __threadfence();
-  nid_finalize<DEVLOOP>(a, n_poses, smem_hist);
+  nid_finalize(a, n_poses, smem_hist);
 }
 
-// DEVLOOP: device-resident solver loop variant (poses from NmDevice, Nelder-Mead step in the finalizing block); kept out of
-// the default instantiation so that its register footprint does not cost the hot loop an occupancy step.
-template <int MODEL, bool F32, bool DEVLOOP>
+template <int MODEL, bool F32>
 __global__ void __launch_bounds__(NID_THREADS) nid_hist_exact_kernel(const __grid_constant__ NidArgs a) {
   extern __shared__ int smem_hist[];
   __shared__ bool s_is_last;
-  const int n_poses = n_poses_of<DEVLOOP>(a);
-  if (n_poses == 0) return;  // device-resident loop: the solver has finished
+  const int n_poses = a.n_poses;
   const int per_copy = n_poses * a.nb;
   if (a.timeline && threadIdx.x == 0 && blockIdx.x == 0) a.timeline[0] = global_ns();
   for (int i = threadIdx.x; i < a.copies * per_copy; i += blockDim.x) smem_hist[i] = 0;
@@ -532,13 +431,13 @@ __global__ void __launch_bounds__(NID_THREADS) nid_hist_exact_kernel(const __gri
     }
     const int lb = lidar_bin_of(w, a.bins);
     for (int p = 0; p < n_poses; p++) {
-      const int ib = classify_exact<MODEL>(a, pose_of<DEVLOOP>(a, p), x, y, z);
+      const int ib = classify_exact<MODEL>(a, a.pose[p], x, y, z);
       if (ib >= 0) {
         atomicAdd(&my_hist[p * a.nb + ib + lb * a.bins], 1);  // :49 hist(image_bin, lidar_bin)++
       }
     }
   }
-  nid_block_epilogue<DEVLOOP>(a, n_poses, smem_hist, &s_is_last);
+  nid_block_epilogue(a, n_poses, smem_hist, &s_is_last);
 }
 
 constexpr int NID_QUEUE = 64;  // per-warp queue of (point, pose) pairs waiting for the exact path
@@ -553,13 +452,13 @@ struct FilterWarp {
   unsigned int lt_mask;
 };
 
-template <int MODEL, bool DEVLOOP>
+template <int MODEL>
 __device__ __forceinline__ void filter_drain32(const NidArgs& a, FilterWarp& w, const float4* __restrict__ pts, int first, int count) {
   if (w.lane < count) {  // entries [first, first+count), count <= 32: one deferred (point, pose) per lane, exact path
     const unsigned int i = w.q_idx[first + w.lane];
     const int p = w.q_pose[first + w.lane];
     const float4 q = __ldg(pts + i);
-    const int ib = classify_exact<MODEL>(a, pose_of<DEVLOOP>(a, p), q.x, q.y, q.z);
+    const int ib = classify_exact<MODEL>(a, a.pose[p], q.x, q.y, q.z);
     if (ib >= 0) atomicAdd(&w.my_hist[p * a.nb + ib + lidar_bin_of(q.w, a.bins) * a.bins], 1);
   }
 }
@@ -578,7 +477,7 @@ __device__ __forceinline__ void filter_load_tile(const float4* __restrict__ pts,
   }
 }
 
-template <int MODEL, int K, bool DEVLOOP>
+template <int MODEL, int K>
 __device__ __forceinline__ void filter_tile(const NidArgs& a, int n_poses, FilterWarp& w, const float4* __restrict__ pts, unsigned int tile, unsigned int end, const float4 (&q)[K]) {
   float px[K], py[K], pz[K], pa[K];
   int lboff[K];
@@ -599,7 +498,7 @@ __device__ __forceinline__ void filter_tile(const NidArgs& a, int n_poses, Filte
     int verdict[K];
     unsigned int unc_bits = 0, ok_bits = 0;
     if (p < n_poses) {
-      const float* __restrict__ P = pose32_of<DEVLOOP>(a, p);
+      const float* __restrict__ P = a.pose32[p];
 #pragma unroll
       for (int j = 0; j < K; j++) {
         int vd = classify_fast<MODEL>(a, P, px[j], py[j], pz[j], pa[j]);
@@ -632,7 +531,7 @@ __device__ __forceinline__ void filter_tile(const NidArgs& a, int n_poses, Filte
             w.qn += __popc(m);
             __syncwarp();
             if (w.qn >= 32) {
-              filter_drain32<MODEL, DEVLOOP>(a, w, pts, w.qn - 32, 32);
+              filter_drain32<MODEL>(a, w, pts, w.qn - 32, 32);
               w.qn -= 32;
               __syncwarp();
             }
@@ -652,15 +551,14 @@ __device__ __forceinline__ void filter_tile(const NidArgs& a, int n_poses, Filte
 // Work split: the cloud is cut into one contiguous, equally long range per warp (multiple of 32 points), processed as
 // NID_KPT-row tiles (NID_KPT points per lane in registers: pose constants fetched once per tile, NID_KPT independent
 // chains in flight) plus single-row tiles for the remainder, so no warp does a whole extra tile more than another.
-template <int MODEL, bool F32, int NID_KPT, bool DEVLOOP>
+template <int MODEL, bool F32, int NID_KPT>
 __global__ void __launch_bounds__(NID_THREADS) nid_hist_filter_kernel(const __grid_constant__ NidArgs a) {
   extern __shared__ int smem_hist[];
   __shared__ bool s_is_last;
   __shared__ unsigned int q_idx[NID_THREADS / 32][NID_QUEUE];
   __shared__ unsigned char q_pose[NID_THREADS / 32][NID_QUEUE];
   static_assert(F32, "the fp32 filter runs on the float4 cloud layout");
-  const int n_poses = n_poses_of<DEVLOOP>(a);
-  if (n_poses == 0) return;  // device-resident loop: the solver has finished
+  const int n_poses = a.n_poses;
   const int per_copy = n_poses * a.nb;
   if (a.timeline && threadIdx.x == 0 && blockIdx.x == 0) a.timeline[0] = global_ns();
   const int warp = threadIdx.x >> 5;
@@ -693,7 +591,7 @@ __global__ void __launch_bounds__(NID_THREADS) nid_hist_filter_kernel(const __gr
       float4 nxt[NID_KPT];
       const bool more = t + 64u * NID_KPT <= end;
       if (more) filter_load_tile<NID_KPT>(pts, t + 32u * NID_KPT, end, w.lane, nxt);
-      filter_tile<MODEL, NID_KPT, DEVLOOP>(a, n_poses, w, pts, t, end, q4);
+      filter_tile<MODEL, NID_KPT>(a, n_poses, w, pts, t, end, q4);
       t += 32u * NID_KPT;
       if (more) {
 #pragma unroll
@@ -706,13 +604,13 @@ __global__ void __launch_bounds__(NID_THREADS) nid_hist_filter_kernel(const __gr
     while (t < end) {
       const bool more = t + 32u < end;
       if (more) filter_load_tile<1>(pts, t + 32u, end, w.lane, n1);
-      filter_tile<MODEL, 1, DEVLOOP>(a, n_poses, w, pts, t, end, q1);
+      filter_tile<MODEL, 1>(a, n_poses, w, pts, t, end, q1);
       t += 32u;
       if (more) q1[0] = n1[0];
     }
   }
-  if (w.qn > 0) filter_drain32<MODEL, DEVLOOP>(a, w, pts, 0, w.qn);
-  nid_block_epilogue<DEVLOOP>(a, n_poses, smem_hist, &s_is_last);
+  if (w.qn > 0) filter_drain32<MODEL>(a, w, pts, 0, w.qn);
+  nid_block_epilogue(a, n_poses, smem_hist, &s_is_last);
 }
 
 // debug / test kernel: runs BOTH paths on every (point, pose) and counts, in a.dbg:

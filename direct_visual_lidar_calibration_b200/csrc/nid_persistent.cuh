@@ -29,12 +29,14 @@
 // Several bags per GPU: the grid is partitioned over the bags in proportion to their sizes (one tail for all bags).
 #pragma once
 
+#include <cfloat>
 #include <cstdint>
 
 #include "exact_classify.cuh"
 #include "lean_filter.cuh"
 #include "lean_filter2.cuh"
 #include "nid_kernels.cuh"
+#include "nm_machine.cuh"
 
 namespace vlcal {
 

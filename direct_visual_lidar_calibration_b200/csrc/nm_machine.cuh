@@ -1,9 +1,8 @@
 // nm_machine.cuh -- dfo::NelderMead<N> (reference: include/dfo/nelder_mead.hpp:32-113) as a resumable state machine.
 //
-// The same __host__ __device__ code drives (a) the host solver loop (host_math.hpp) and (b) the device-resident loop in
-// which the finalizing block of the NID kernel consumes the scores of the batch it has just computed and emits the next
-// batch of candidate poses without returning to the host (nid_kernels.cuh).  Decisions are those of the serial
-// reference, evaluation for evaluation:
+// The host solver loop (host_math.hpp) steps it; the persistent kernel (nid_persistent.cuh) keeps its solver state in the
+// same struct and steps it with a warp-parallel twin of step().  Decisions are those of the serial reference, evaluation
+// for evaluation:
 //   - libstdc++'s insertion-sort order for std::sort on <= 16 elements (ties and NaNs land where the reference puts them)
 //   - the centroid xo is evaluated although its value is never used (:58)
 //   - the "contraction" point lies on the reflected side, xo + rho (xo - worst) (:75)

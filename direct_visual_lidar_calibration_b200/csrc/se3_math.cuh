@@ -1,4 +1,4 @@
-// se3_math.cuh -- __host__ __device__ SE(3) helpers shared by the host solver and the device-resident solver loop:
+// se3_math.cuh -- __host__ __device__ SE(3) helpers of the host solver (the persistent kernel repeats their operations):
 //   gtsam::Pose3::Expmap            (call sites src/vlcal/calib/visual_camera_calibration.cpp:104,129; GTSAM 4.2a9)
 //   Eigen::Isometry3d * Isometry3d  (visual_camera_calibration.cpp:104)
 // 4x4 matrices are column-major (Eigen::Isometry3d::matrix().data()).  Arithmetic goes through exact_math.cuh, so the

@@ -409,12 +409,8 @@ int vlcal_render_overlay(
  *     Needs float4 clouds, bins <= 32, one camera / image size / device, no host all-reduce callback; VLCAL_ERR_UNSUPPORTED
  *     otherwise.  params.callback is delivered after the solve from the evaluation trace, in the reference's order.
  *   1 host loop: one launch per Nelder-Mead batch, scores published to mapped host memory, host polls.
- *   2 device-resident loop (one local bag; scores local or summed by the in-kernel peer exchange): the state machine
- *     advances inside the kernel's finalizing block, launches are enqueued back to back; VLCAL_ERR_UNSUPPORTED otherwise.
- * Both loops run the same state machine (bit-identical trajectory, tests/test_gpu_parity.py).  At the C2 size the host
- * loop was measured the faster one (stepping the machine + Expmap on one SM costs more than the host round trip it
- * removes), hence the default; with mode 2 params.callback is delivered from the evaluation trace, in
- * the reference's order, up to one chunk of launches late. */
+ * Both loops walk the same Nelder-Mead trajectory, bit for bit (tests/test_gpu_parity.py).  Any other mode, 2 included,
+ * is VLCAL_ERR_INVALID_ARGUMENT. */
 int vlcal_nid_set_solver_mode(int mode);
 /* test hook: with recording armed on the calling thread (enable != 0; off by default, 0 turns it off again), every inner
  * solve (vlcal_estimate_pose_nelder_mead*, any solver mode) run on that thread keeps its evaluations as the best-cost

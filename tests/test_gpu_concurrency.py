@@ -391,7 +391,7 @@ def _synthetic_bag(n, cfg):
 
 
 def _case_solves():
-    """Whole inner solves per thread with the solve trace armed in each thread, in solver modes 0, 1 and 2 (set
+    """Whole inner solves per thread with the solve trace armed in each thread, in solver modes 0 and 1 (set
     process-wide before the threads start), then one calibrate on two bags per thread."""
     V, O = _libs()
     bags = [_synthetic_bag(n, cfg=3 + k) for k, n in enumerate((200_000, 12_000, 8_000))]
@@ -415,7 +415,7 @@ def _case_solves():
             _VC.record_solve_trace(False)
 
     try:
-        for mode in (0, 1, 2):
+        for mode in (0, 1):
             V.set_solver_mode(mode)
             serial = [solve(k) for k in range(len(bags))]
             for (T, x, costs, trace), ref in zip(serial, oracle_traces):
@@ -537,7 +537,7 @@ _CASES = {
     "score_poses": _case_score_poses_disjoint_lists,
     "mode_b": _case_mode_b,
     "legacy_stream": _case_legacy_stream_entry_points,
-    "solves": _case_solves,
+    "solves_auto_and_host": _case_solves,
     "errors": _case_error_isolation,
     "churn": _case_churn,
 }

@@ -1,7 +1,6 @@
 """GPU edge suite of the round-1 NID kernels (csrc/nid_kernels.cuh): nid_hist_exact_kernel, nid_hist_filter_kernel at 2
-and 4 points per lane, their device-resident (DEVLOOP) instances and nid_finalize.  They score every context the
-persistent kernel refuses -- double-layout clouds, 33 ... 128 bins, cameras without the lean classifier, an attached peer
-exchange -- and run solver modes 1 and 2.
+and 4 points per lane, and nid_finalize.  They score every context the persistent kernel refuses -- double-layout clouds,
+33 ... 128 bins, cameras without the lean classifier, an attached peer exchange -- and run solver mode 1.
 
 Bar (the one of the persistent kernel's suite): integer histograms bit-identical to oracle.nid_calculate, NID within 1e-12
 of the oracle with NaN exactly where the oracle has NaN, and bit-identical results across kernel instances and across ways
@@ -46,11 +45,11 @@ def launches(P, bins):
 
 def geometry(P, bins):
     """The switches of one launch of P <= max_poses poses: histogram copies, the finalizer's split over warps, warps per
-    pose and whether pass 1's counts stay in registers for pass 2; and whether the device-resident loop is allowed."""
+    pose and whether pass 1's counts stay in registers for pass 2."""
     nb = bins * bins
     split = nb <= 1024
     wpp = max(1, 8 // P) if split else 1
-    return {"max_poses": max_poses(bins), "devloop": max_poses(bins) == 8, "copies": max(1, min(2, NID_HIST_TARGET // (P * nb * 4))),
+    return {"max_poses": max_poses(bins), "copies": max(1, min(2, NID_HIST_TARGET // (P * nb * 4))),
             "split": split, "wpp": wpp, "single": nb <= wpp * 32 * 8}
 
 
@@ -70,7 +69,7 @@ def test_cases_cross_every_switch_of_the_launch_geometry():
                 for k, v in g.items():
                     seen.setdefault(k, set()).add(v)
     assert seen["max_poses"] == {8, 7, 6, 3, 2, 1}
-    assert seen["devloop"] == seen["split"] == seen["single"] == {True, False}
+    assert seen["split"] == seen["single"] == {True, False}
     assert seen["copies"] == {1, 2} and seen["wpp"] == {1, 2, 4, 8}
     assert [max_poses(b) for b in (55, 56, 64, 90, 91, 110, 111, 128)] == [8, 7, 6, 3, 2, 2, 1, 1]
     # the pairs either side of the single register pass: 22 / 23 bins at two warps per pose, 16 / 17 at one, 32 / 33 at split
@@ -343,30 +342,17 @@ def _solve_setup(V, bag, bins, iters):
 
 
 @pytest.mark.parametrize("bins", [33, 55])
-def test_host_loop_and_device_loop_above_32_bins(gpu, oracle, bins):
-    """Mode 1 (one round-1 launch per batch) and mode 2 (the DEVLOOP filter instance, machine stepped by the finalizer)."""
+def test_host_loop_above_32_bins(gpu, oracle, bins):
+    """Mode 1 (one round-1 launch per batch) at bin counts the persistent kernel refuses, 8 poses per launch."""
     V = gpu
     bag = _synthetic_bag(20_000, cfg=3)
     cam_args, cam, params = _solve_setup(V, bag, bins, 25)
     ds = [V.VisualLiDARData(bag["image"], bag["points"], bag["intensities"])]
-    out = _solve_modes(V, cam, ds, bag["T_init"], params, modes=(1, 2))
-    _assert_same_solve(out[1], out[2])
+    out = _solve_modes(V, cam, ds, bag["T_init"], params, modes=(1,))
     ref = _oracle_solve(oracle, cam_args, ds, bag["T_init"], 25, bins=bins)
-    T, r, _, tr = out[2]
+    T, r, _, tr = out[1]
     assert np.array_equal(r["x"], ref["x"]) and r["num_evaluations"] == ref["num_evaluations"] and np.abs(T - ref["T"]).max() == 0.0
     _assert_trace_is_oracles(tr, ref["trace"])
-
-
-def test_device_loop_refuses_56_bins(gpu):
-    """56 bins leave room for 7 poses per launch, not the 8 of a device-resident batch: an error, not another path."""
-    V = gpu
-    bag = _synthetic_bag(5_000, cfg=3)
-    _, cam, params = _solve_setup(V, bag, 56, 5)
-    assert max_poses(56) == 7
-    ds = [V.VisualLiDARData(bag["image"], bag["points"], bag["intensities"])]
-    with pytest.raises(V.VlcalError) as e:
-        _solve_modes(V, cam, ds, bag["T_init"], params, modes=(2,))
-    assert e.value.code == -6
 
 
 @pytest.mark.parametrize("bins", [64, 128])
@@ -409,15 +395,14 @@ def _double_layout_bag(n, cfg, seed):
     return bag
 
 
-def test_double_layout_solve_host_and_device_loop(gpu, oracle):
+def test_double_layout_solve_auto_and_host_loop(gpu, oracle):
     V = gpu
     bag = _double_layout_bag(15_000, 5, 1700)
     cam_args, cam, params = _solve_setup(V, bag, 16, 20)
     ds = [V.VisualLiDARData(bag["image"], bag["points"], bag["intensities"])]
     assert not V.CostCalculatorNID(cam, ds[0]).points_are_f32
-    out = _solve_modes(V, cam, ds, bag["T_init"], params, modes=(0, 1, 2))  # 0: the persistent kernel refuses, host loop
+    out = _solve_modes(V, cam, ds, bag["T_init"], params, modes=(0, 1))  # 0: the persistent kernel refuses, host loop
     _assert_same_solve(out[0], out[1])
-    _assert_same_solve(out[1], out[2])
     ref = _oracle_solve(oracle, cam_args, ds, bag["T_init"], 20)
     T, r, _, tr = out[1]
     assert np.array_equal(r["x"], ref["x"]) and np.abs(T - ref["T"]).max() == 0.0

@@ -123,6 +123,20 @@ def test_batched_nelder_mead_follows_the_serial_trajectory(vlcal, oracle, name, 
     assert res["num_evaluations_computed"] >= res["num_evaluations"]
 
 
+def test_solver_mode_accepts_auto_host_and_persistent_only(vlcal):
+    """Modes 0, 1 and 3 select a solver loop; 2 (the round-1 device-resident loop, removed) is refused, not remapped."""
+    try:
+        for mode in (0, 1, 3):
+            vlcal.set_solver_mode(mode)
+        for mode in (2, -1, 4):
+            with pytest.raises(vlcal.VlcalError) as e:
+                vlcal.set_solver_mode(mode)
+            assert e.value.code == -1  # VLCAL_ERR_INVALID_ARGUMENT
+            assert ("device-resident loop was removed" in e.value.message) == (mode == 2), e.value.message
+    finally:
+        vlcal.set_solver_mode(0)
+
+
 def test_default_params_match_reference(vlcal):
     p = vlcal.VisualCameraCalibrationParams().to_c()
     assert (p.max_outer_iterations, p.max_inner_iterations, p.nid_bins) == (10, 256, 16)
