@@ -231,13 +231,14 @@ def estimate_pose_on_costs(costs, init_T_camera_lidar, params: VisualCameraCalib
     handles = (C.c_void_p * len(costs))(*[c.handle for c in costs])
 
     def _pose_cb(Tp, cost, _user):
-        if callback:
-            callback(colmajor_to_T(np.ctypeslib.as_array(Tp, shape=(16,)))[0], float(cost))
+        callback(colmajor_to_T(np.ctypeslib.as_array(Tp, shape=(16,)))[0], float(cost))
 
     def _allreduce(vals, count, _user):
         allreduce(np.ctypeslib.as_array(vals, shape=(count,)))
 
-    cb = _lib.POSE_CALLBACK(_pose_cb)
+    # no callback: the null one, so the library knows that nobody observes the evaluations (it then skips scoring the
+    # centroid of every iteration, whose value feeds no decision)
+    cb = _lib.POSE_CALLBACK(_pose_cb) if callback else _lib.POSE_CALLBACK()
     ar = _lib.ALLREDUCE_FN(_allreduce) if allreduce else _lib.ALLREDUCE_FN()
     p = params.to_c()
     T0 = T_to_colmajor(init_T_camera_lidar)

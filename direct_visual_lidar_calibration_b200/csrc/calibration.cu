@@ -3,7 +3,8 @@
 //
 // Same decisions as the reference (outer loop, culling at the start pose of every inner solve, one cost object per
 // bag, dfo::NelderMead<6> with the calibration parameters), but every Nelder-Mead iteration scores its candidate
-// poses {xo, xr, xe, xc} in ONE batched kernel launch per bag, and bags run concurrently on their own streams.
+// poses {xr, xe, xc} (plus the centroid xo when its value can be observed, run_inner_solve) in ONE batched kernel launch
+// per bag, and bags run concurrently on their own streams.
 #include <chrono>
 #include <cstring>
 #include <vector>
@@ -103,12 +104,19 @@ int run_inner_solve(
   for (int i = 1; i < n_ctxs; i++) same_px = same_px && ctxs[i]->p2p == ctxs[0]->p2p;
   const bool px_fused = n_ctxs >= 1 && ctx_exchange_is_fused(ctxs[0]);
   const bool pk_ok = n_ctxs >= 1 && params->max_inner_iterations >= 0 && same_px && (allreduce == nullptr || px_fused) && pk_supported(ctxs, n_ctxs);
+  // The centroid xo of an iteration (nelder_mead.hpp:58) never feeds a decision; its value reaches a user only as a side
+  // effect of the objective: the best-cost callback or the recorded solve trace.  Without either, the iteration batches
+  // score {xr, xe, xc} only.  Several ranks (a host all-reduce or an attached peer exchange) keep scoring it: every rank
+  // must issue batches of the same size, and a rank with a callback would otherwise wait for words the others never send.
+  bool px_any = false;
+  for (int i = 0; i < n_ctxs; i++) px_any = px_any || ctx_exchange_is_fused(ctxs[i]);
+  const bool score_centroid = callback != nullptr || g_record_solve_trace || allreduce != nullptr || px_any;
   if (g_solver_mode == 3 && !pk_ok) {
     set_last_error("persistent solve requested but these contexts need the host loop (double-layout cloud / bins > 32 / camera without the lean classifier / host all-reduce / mixed image sizes)");
     return VLCAL_ERR_UNSUPPORTED;
   }
   if (pk_ok && (g_solver_mode == 0 || g_solver_mode == 3)) {
-    return pk_solve(ctxs, n_ctxs, params, init_T, callback, user, T_out, nm_result);
+    return pk_solve(ctxs, n_ctxs, params, init_T, callback, user, T_out, nm_result, score_centroid);
   }
   if (n_ctxs > 1 && px_fused) {
     // the round-1 kernels exchange one bag per rank; with several local bags only the persistent kernel sums in-kernel
@@ -125,7 +133,7 @@ int run_inner_solve(
   const double x0[6] = {0, 0, 0, 0, 0, 0};
   auto f = [&](const double* xs, int count, double* ys) { obj.evaluate(xs, count, ys); };
   auto ob = [&](const double* x, double y) { obj.observe(x, y); };
-  const host::NelderMeadResult r = host::nelder_mead(6, f, ob, x0, nm, /*speculate=*/true);  // :126-127
+  const host::NelderMeadResult r = host::nelder_mead(6, f, ob, x0, nm, /*speculate=*/true, score_centroid);  // :126-127
   if (obj.status != VLCAL_OK) return obj.status;
 
   double E[16];

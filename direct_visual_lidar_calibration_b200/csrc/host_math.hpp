@@ -91,11 +91,12 @@ struct NelderMeadResult {  // optimizer.hpp:8-20
 // BatchF:   void(const double* xs /*count x n*/, int count, double* ys)
 // ObserveF: void(const double* x, double y)   -- called once per reference evaluation, in reference order
 // (`speculate` is kept for call-site readability: candidates are always scored one batch per iteration; only the
-// values the reference would have requested are consumed.)
+// values the reference would have requested are consumed.)  score_centroid = false: iteration batches leave out the
+// centroid, whose value then never reaches `observe` (NmMachine::begin); for callers that read no side effects.
 template <typename BatchF, typename ObserveF>
-NelderMeadResult nelder_mead(int n, BatchF&& f, ObserveF&& observe, const double* x0, const NelderMeadParams& params, bool /*speculate*/) {
+NelderMeadResult nelder_mead(int n, BatchF&& f, ObserveF&& observe, const double* x0, const NelderMeadParams& params, bool /*speculate*/, bool score_centroid = true) {
   NmMachine nm;
-  nm.begin(n, params, x0);
+  nm.begin(n, params, x0, score_centroid);
   std::vector<double> xs(static_cast<size_t>(NM_MAX_N + 1) * n), ys(NM_MAX_N + 1);
   while (nm.phase != 3) {
     for (int k = 0; k < nm.n_cand; k++) std::memcpy(&xs[static_cast<size_t>(k) * n], &nm.cand[k][1], sizeof(double) * n);

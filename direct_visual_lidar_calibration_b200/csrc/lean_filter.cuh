@@ -289,8 +289,9 @@ VL_HD float lean_delta_row_spread(const float* __restrict__ a, const float* __re
 // largest gate entry to the other poses is smallest, ties to the lowest index, so every block, every rank and the host
 // pick the same pose.  The bound of the delta step holds for any anchor; this choice puts as many batches as possible
 // inside the gate and keeps the remainder term, which grows with the squared distance to the anchor, small.  For a
-// Nelder-Mead iteration {xo, xr, xe, xc} (s = 0, 1, 2, 1/2 along one line) it is xr: the farthest pose is |diff| away
-// instead of 2 |diff|, and the squared offsets sum to 2.25 |diff|^2 instead of 5.25.  For the initial simplex it is x0.
+// Nelder-Mead iteration {xr, xe, xc, xo} (s = 1, 2, 1/2, 0 along one line) it is xr, index 0: the farthest pose is
+// |diff| away instead of 2 |diff|, and the squared offsets sum to 2.25 |diff|^2 instead of 5.25 (1.25 |diff|^2 when the
+// centroid xo is not scored, nm_machine.cuh).  For the initial simplex it is x0.
 // pk_delta_rows computes the same scores warp-parallel (max and min are exact, so any grouping gives the same bits).
 VL_HD float lean_delta_anchor_score(const double (*__restrict__ T)[12], int n, int i) {
   float s = 0.0f;

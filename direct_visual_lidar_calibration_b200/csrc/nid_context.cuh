@@ -156,10 +156,11 @@ int nid_wait(vlcal_nid_ctx* ctx, double* nid_out, int32_t* hist_out);
 // persistent cooperative kernel (nid_persistent.cu): can these contexts (bags of one camera on one device) run on it?
 bool pk_supported(vlcal_nid_ctx* const* ctxs, int n_ctxs);
 // a whole Nelder-Mead inner solve (visual_camera_calibration.cpp:103-129) in one launch; sums over the peer exchange
-// attached to ctxs[0] when it spans several ranks
+// attached to ctxs[0] when it spans several ranks.  score_centroid: the iteration batches score xo and the kernel
+// writes the evaluation trace (NmMachine::begin)
 int pk_solve(
   vlcal_nid_ctx* const* ctxs, int n_ctxs, const vlcal_calib_params* params, const double init_T[16], vlcal_pose_callback callback, void* user, double T_out[16],
-  vlcal_nm_result* nm_result);
+  vlcal_nm_result* nm_result, bool score_centroid);
 // sum over the contexts of calculate(T_p) for a pose list of any length, one launch (hist_out: bag 0's joint histograms)
 int pk_score_poses(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_colmajor, int n_poses, double* nid_out, int32_t* hist_out);
 

@@ -215,7 +215,7 @@ int pk_grid_size(const PkGeom& g, vlcal_nid_ctx* const* ctxs, int n_ctxs) {
 
 int pk_solve(
   vlcal_nid_ctx* const* ctxs, int n_ctxs, const vlcal_calib_params* params, const double init_T[16], vlcal_pose_callback callback, void* user, double T_out[16],
-  vlcal_nm_result* nm_result) {
+  vlcal_nm_result* nm_result, bool score_centroid) {
   vlcal_nid_ctx* c0 = ctxs[0];
   VL_CUDA(cudaSetDevice(c0->device));
   const int kpt = pk_points_per_lane(c0);
@@ -239,8 +239,9 @@ int pk_solve(
   VL_CUDA(cudaMemsetAsync(scratch.p, 0, L.total, c0->stream));
 
   // host-visible outcome: result + done / error words + evaluation trace, one pinned allocation
-  // n + 1 evaluations of the initial simplex, then at most n + 3 per iteration: xo, xr, xc and the n shrunk vertices
-  const int trace_cap = 7 + std::max(0, params->max_inner_iterations) * 9;
+  // n + 1 evaluations of the initial simplex, then at most n + 3 per iteration: xo, xr, xc and the n shrunk vertices.
+  // Without the centroid nothing replays the trace (run_inner_solve), so block 0 writes none.
+  const int trace_cap = score_centroid ? 7 + std::max(0, params->max_inner_iterations) * 9 : 0;
   const size_t trace_bytes = sizeof(double) * (NM_MAX_N + 1) * static_cast<size_t>(trace_cap);
   const size_t head_bytes = (sizeof(PkResult) + sizeof(PkSolve) + 64 + 255) & ~static_cast<size_t>(255);
   PinBuf host;
@@ -261,7 +262,7 @@ int pk_solve(
   nm.max_iterations = params->max_inner_iterations;
   std::memset(static_cast<void*>(h_solve), 0, sizeof(PkSolve));
   const double x0[6] = {0, 0, 0, 0, 0, 0};
-  h_solve->nm.begin(6, nm, x0);  // :126 optimize(f, Zero)
+  h_solve->nm.begin(6, nm, x0, score_centroid);  // :126 optimize(f, Zero)
   std::memcpy(h_solve->init_T, init_T, sizeof(h_solve->init_T));
   char* sp = static_cast<char*>(scratch.p);
   VL_CUDA(cudaMemcpyAsync(sp + L.solve, h_solve, sizeof(PkSolve), cudaMemcpyHostToDevice, c0->stream));

@@ -324,19 +324,19 @@ static __device__ void nm_warp_loop_top(NmMachine& s, int lane) {
     nm_warp_finish(s, lane);
     return;
   }
-  // :57, :60, :66, :75  xo, xr, xe, xc
+  // :57, :60, :66, :75  xo, xr, xe, xc -> cand = {xr, xe, xc, xo} (xo scored only when s.score_centroid)
   if (mine) {
     xd sum(0.0);
     for (int k = 0; k < n; k++) sum = sum + xd(s.x[k][lane]);
     const xd xo = sum / xd(static_cast<double>(n));
     const xd diff = xo - xd(s.x[n][lane]);
-    s.cand[0][lane] = xo.v;
-    s.cand[1][lane] = (xo + xd(s.params.alpha) * diff).v;
-    s.cand[2][lane] = (xo + xd(s.params.gamma) * diff).v;
-    s.cand[3][lane] = (xo + xd(s.params.rho) * diff).v;
+    s.cand[0][lane] = (xo + xd(s.params.alpha) * diff).v;
+    s.cand[1][lane] = (xo + xd(s.params.gamma) * diff).v;
+    s.cand[2][lane] = (xo + xd(s.params.rho) * diff).v;
+    s.cand[3][lane] = xo.v;
   }
   if (lane == 0) {
-    s.n_cand = 4;
+    s.n_cand = s.score_centroid ? 4 : 3;
     s.phase = 1;
   }
   __syncwarp();
@@ -368,30 +368,37 @@ static __device__ __noinline__ void nm_warp_step(NmMachine& s, const double* ys,
     nm_warp_loop_top_dispatch(s, lane);
   } else if (phase == 1) {
     const double f0 = s.x[0][0], fn1 = s.x[n - 1][0], fn = s.x[n][0];
-    const double y0 = ys[0], y1 = ys[1], y2 = ys[2], y3 = ys[3];
+    // scores of cand = {xr, xe, xc, xo}
+    const double yr = ys[0], ye = ys[1], yc = ys[2];
+    const bool score_centroid = s.score_centroid != 0;
     __syncwarp();
     if (lane == 0) {
-      s.cand[0][0] = y0;
-      s.cand[1][0] = y1;
+      s.cand[0][0] = yr;
+      if (score_centroid) s.cand[3][0] = ys[3];
     }
     __syncwarp();
-    nm_warp_observe(s, lane, s.cand[0], y0);  // :58 evaluated, never used in a decision
-    nm_warp_observe(s, lane, s.cand[1], y1);  // :61
-    bool shrink = false;
-    if (f0 <= y1 && y1 < fn1) {  // :63-64
-      if (mine) s.x[n][lane] = s.cand[1][lane];
-    } else if (y1 < f0) {  // :65-73 expansion
-      if (lane == 0) s.cand[2][0] = y2;
+    if (score_centroid) {
+      nm_warp_observe(s, lane, s.cand[3], ys[3]);  // :58 evaluated, never used in a decision
+    } else {
+      if (lane == 0) s.num_evaluations++;  // :58 requested by the reference; nobody reads its value
       __syncwarp();
-      nm_warp_observe(s, lane, s.cand[2], y2);
-      const int pick = (y2 < y1) ? 2 : 1;
+    }
+    nm_warp_observe(s, lane, s.cand[0], yr);  // :61
+    bool shrink = false;
+    if (f0 <= yr && yr < fn1) {  // :63-64
+      if (mine) s.x[n][lane] = s.cand[0][lane];
+    } else if (yr < f0) {  // :65-73 expansion
+      if (lane == 0) s.cand[1][0] = ye;
+      __syncwarp();
+      nm_warp_observe(s, lane, s.cand[1], ye);
+      const int pick = (ye < yr) ? 1 : 0;
       if (mine) s.x[n][lane] = s.cand[pick][lane];
     } else {  // :74-86
-      if (lane == 0) s.cand[3][0] = y3;
+      if (lane == 0) s.cand[2][0] = yc;
       __syncwarp();
-      nm_warp_observe(s, lane, s.cand[3], y3);
-      if (y3 < fn) {
-        if (mine) s.x[n][lane] = s.cand[3][lane];
+      nm_warp_observe(s, lane, s.cand[2], yc);
+      if (yc < fn) {
+        if (mine) s.x[n][lane] = s.cand[2][lane];
       } else {
         shrink = true;
         if (mine) {

@@ -4,14 +4,18 @@
 // same struct and steps it with a warp-parallel twin of step().  Decisions are those of the serial reference, evaluation
 // for evaluation:
 //   - libstdc++'s insertion-sort order for std::sort on <= 16 elements (ties and NaNs land where the reference puts them)
-//   - the centroid xo is evaluated although its value is never used (:58)
+//   - the centroid xo is requested although its value is never used in a decision (:58): it is counted as a reference
+//     evaluation always, but scored only when its value can be observed (begin(): score_centroid)
 //   - the "contraction" point lies on the reflected side, xo + rho (xo - worst) (:75)
 //   - the shrink step uses rho, not sigma (:82)
 //   - convergence = sum over the N coordinates of sum_k (x_k - mean)^2 < threshold, no 1/n (:105-113)
 //   - the result is x[0] as of the last sort (:99-100), num_iterations the last loop index (:50)
-// {xo, xr, xe, xc} are affine in the sorted simplex, so they are known before any is scored: one batch of 4 per
-// iteration (N+1 for the initial simplex, N for a shrink); only the values the reference would have requested are
-// consumed, and `obs_*` lists them in the reference's order so that the objective's side effects can be replayed.
+// {xo, xr, xe, xc} are affine in the sorted simplex, so they are known before any is scored: one batch per iteration
+// (N+1 for the initial simplex, N for a shrink); only the values the reference would have requested are consumed, and
+// `obs_*` lists them in the reference's order so that the objective's side effects can be replayed.  An iteration batch
+// is cand = {xr, xe, xc, xo}: 4 poses when the caller observes the objective's side effects (a best-cost callback, a
+// recorded trace, ranks that must issue equal batches), else 3 -- xo's value then reaches nobody, so it is not scored,
+// and its entry is left out of `obs_*`.  Every score depends on its own pose alone, so both give the same trajectory.
 // All arithmetic goes through exact_math.cuh (no FMA contraction on either side).
 #pragma once
 
@@ -34,6 +38,7 @@ struct NmParams {  // nelder_mead.hpp:11-22
 struct NmMachine {
   // configuration
   int n;
+  int score_centroid;  // iteration batches score xo too (4 poses instead of 3)
   NmParams params;
   // state
   int phase;      // 0 initial simplex pending, 1 iteration batch pending, 2 shrink batch pending, 3 finished
@@ -62,9 +67,10 @@ struct NmMachine {
     num_evaluations++;
   }
 
-  // :35-46 initial simplex -> first batch
-  VL_HD void begin(int n_, const NmParams& p, const double* x0) {
+  // :35-46 initial simplex -> first batch.  score_centroid_: whether the caller reads xo's value (through obs_*)
+  VL_HD void begin(int n_, const NmParams& p, const double* x0, bool score_centroid_ = true) {
     n = n_;
+    score_centroid = score_centroid_ ? 1 : 0;
     params = p;
     phase = 0, it = 0, converged = 0, num_iterations = 0;
     num_evaluations = num_batches = num_evaluations_computed = 0;
@@ -133,18 +139,18 @@ struct NmMachine {
         return;
       }
     }
-    // :57, :60, :66, :75  xo, xr, xe, xc -> cand[0..3]
+    // :57, :60, :66, :75  xo, xr, xe, xc -> cand = {xr, xe, xc, xo}
     for (int d = 0; d < m; d++) {
       xd s(0.0);
       for (int k = 0; k < n; k++) s = s + xd(x[k][d]);
       const xd xo = s / xd(static_cast<double>(n));
       const xd diff = xo - xd(x[n][d]);
-      cand[0][d] = xo.v;
-      cand[1][d] = (xo + xd(params.alpha) * diff).v;
-      cand[2][d] = (xo + xd(params.gamma) * diff).v;
-      cand[3][d] = (xo + xd(params.rho) * diff).v;
+      cand[0][d] = (xo + xd(params.alpha) * diff).v;
+      cand[1][d] = (xo + xd(params.gamma) * diff).v;
+      cand[2][d] = (xo + xd(params.rho) * diff).v;
+      cand[3][d] = xo.v;
     }
-    n_cand = 4;
+    n_cand = score_centroid ? 4 : 3;
     phase = 1;
   }
 
@@ -163,23 +169,28 @@ struct NmMachine {
       }
       loop_top();
     } else if (phase == 1) {
-      double* xo = cand[0];
-      double* xr = cand[1];
-      double* xe = cand[2];
-      double* xc = cand[3];
-      xo[0] = ys[0], xr[0] = ys[1];
-      observe(xo, xo[0]);  // :58 evaluated, value never used in a decision
+      double* xr = cand[0];
+      double* xe = cand[1];
+      double* xc = cand[2];
+      double* xo = cand[3];
+      xr[0] = ys[0];
+      if (score_centroid) {
+        xo[0] = ys[3];
+        observe(xo, xo[0]);  // :58 evaluated, value never used in a decision
+      } else {
+        num_evaluations++;  // :58 requested by the reference; nobody reads its value
+      }
       observe(xr, xr[0]);  // :61
       bool shrink = false;
       if (x[0][0] <= xr[0] && xr[0] < x[n - 1][0]) {  // :63-64
         for (int d = 0; d < m; d++) x[n][d] = xr[d];
       } else if (xr[0] < x[0][0]) {  // :65-73 expansion
-        xe[0] = ys[2];
+        xe[0] = ys[1];
         observe(xe, xe[0]);
         const double* pick = (xe[0] < xr[0]) ? xe : xr;
         for (int d = 0; d < m; d++) x[n][d] = pick[d];
       } else {  // :74-86
-        xc[0] = ys[3];
+        xc[0] = ys[2];
         observe(xc, xc[0]);
         if (xc[0] < x[n][0]) {
           for (int d = 0; d < m; d++) x[n][d] = xc[d];
