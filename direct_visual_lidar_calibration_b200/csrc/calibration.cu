@@ -92,6 +92,59 @@ struct PoseObjective {
   }
 };
 
+// What a rank of a peer exchange would do on its own: whether its contexts can take the persistent kernel, its solver
+// mode, its number of local bags and its bins.  Packed into one word for p2p_gather.
+struct SolvePlan {
+  bool pk;
+  int mode, n_bags, bins;
+  unsigned long long word() const {
+    return static_cast<unsigned long long>(pk ? 1 : 0) | static_cast<unsigned long long>(mode & 0xff) << 8 | static_cast<unsigned long long>(n_bags & 0xffff) << 16 |
+           static_cast<unsigned long long>(bins & 0xffff) << 32;
+  }
+  static SolvePlan of(unsigned long long w) {
+    return SolvePlan{(w & 1ull) != 0, static_cast<int>((w >> 8) & 0xff), static_cast<int>((w >> 16) & 0xffff), static_cast<int>((w >> 32) & 0xffff)};
+  }
+  std::string describe() const {
+    return std::string(pk ? "persistent-capable" : "host loop only") + ", solver mode " + std::to_string(mode) + ", " + std::to_string(n_bags) + " bag(s), " +
+           std::to_string(bins) + " bins";
+  }
+};
+
+// The solve-path agreement.  Each rank picks its path from its own bags, but the round-1 exchange (host loop, one bag per
+// rank) and the persistent kernel's exchange ((rank, bag) words, the same number of bags on every rank) only meet their
+// own kind: ranks that chose differently would each wait for words that never come.  So before a solve every rank
+// publishes its plan in one exchange and reads all of them; every rank then decides the same way:
+//   * plans equal: the path each rank would take alone (it is the same everywhere);
+//   * plans differ and every rank holds one bag, with no rank in solver mode 3: all ranks take the host loop (the
+//     round-1 exchange sums one bag per rank whatever the layout, camera or bins);
+//   * otherwise every rank refuses with VLCAL_ERR_UNSUPPORTED, naming the ranks whose plan differs from rank 0's.
+int agree_solve_path(vlcal_p2p* px, cudaStream_t stream, const SolvePlan& mine, bool* host_loop) {
+  *host_loop = false;
+  unsigned long long words[P2P_MAX_RANKS];
+  const int rc = p2p_gather(px, stream, mine.word(), words);
+  if (rc != VLCAL_OK) return rc;
+  bool equal = true, one_bag_each = true, mode3 = false;
+  for (int r = 0; r < px->world; r++) {
+    const SolvePlan p = SolvePlan::of(words[r]);
+    equal = equal && words[r] == words[0];
+    one_bag_each = one_bag_each && p.n_bags == 1;
+    mode3 = mode3 || p.mode == 3;
+  }
+  if (equal) return VLCAL_OK;
+  if (one_bag_each && !mode3) {
+    *host_loop = true;
+    return VLCAL_OK;
+  }
+  std::string differ, plans;
+  for (int r = 0; r < px->world; r++) {
+    if (words[r] != words[0]) differ += (differ.empty() ? "" : ", ") + std::to_string(r);
+    plans += "; rank " + std::to_string(r) + ": " + SolvePlan::of(words[r]).describe();
+  }
+  set_last_error("peer exchange: the ranks' solve plans differ (rank(s) " + differ + " against rank 0" + plans +
+                 "): with several bags per rank, or solver mode 3, every rank needs the same number of bags, bins, layout and mode");
+  return VLCAL_ERR_UNSUPPORTED;
+}
+
 int run_inner_solve(
   vlcal_nid_ctx* const* ctxs, int n_ctxs, const vlcal_calib_params* params, const double init_T[16], vlcal_pose_callback callback, vlcal_allreduce_fn allreduce, void* user,
   double T_out[16], vlcal_nm_result* nm_result) {
@@ -103,7 +156,13 @@ int run_inner_solve(
   bool same_px = true;
   for (int i = 1; i < n_ctxs; i++) same_px = same_px && ctxs[i]->p2p == ctxs[0]->p2p;
   const bool px_fused = n_ctxs >= 1 && ctx_exchange_is_fused(ctxs[0]);
-  const bool pk_ok = n_ctxs >= 1 && params->max_inner_iterations >= 0 && same_px && (allreduce == nullptr || px_fused) && pk_supported(ctxs, n_ctxs);
+  bool pk_ok = n_ctxs >= 1 && params->max_inner_iterations >= 0 && same_px && (allreduce == nullptr || px_fused) && pk_supported(ctxs, n_ctxs);
+  if (px_fused) {
+    bool host_loop = false;
+    const int rc = agree_solve_path(ctxs[0]->p2p, ctxs[0]->stream, SolvePlan{pk_ok, g_solver_mode, n_ctxs, ctxs[0]->bins}, &host_loop);
+    if (rc != VLCAL_OK) return rc;
+    pk_ok = pk_ok && !host_loop;
+  }
   // The centroid xo of an iteration (nelder_mead.hpp:58) never feeds a decision; its value reaches a user only as a side
   // effect of the objective: the best-cost callback or the recorded solve trace.  Without either, the iteration batches
   // score {xr, xe, xc} only.  Several ranks (a host all-reduce or an attached peer exchange) keep scoring it: every rank
@@ -118,11 +177,23 @@ int run_inner_solve(
   if (pk_ok && (g_solver_mode == 0 || g_solver_mode == 3)) {
     return pk_solve(ctxs, n_ctxs, params, init_T, callback, user, T_out, nm_result, score_centroid);
   }
+  // the round-1 kernels exchange one bag per rank; with several local bags only the persistent kernel sums in-kernel, or
+  // a host all-reduce callback sums the host loop's partial sums (the contexts then run without their exchange)
+  std::vector<vlcal_p2p*> detached;
   if (n_ctxs > 1 && px_fused) {
-    // the round-1 kernels exchange one bag per rank; with several local bags only the persistent kernel sums in-kernel
-    set_last_error("several local bags with an attached peer exchange need the persistent solve (solver mode 0 / 3)");
-    return VLCAL_ERR_UNSUPPORTED;
+    if (!allreduce) {
+      set_last_error("several local bags with an attached peer exchange need the persistent solve (solver mode 0 / 3) or a host all-reduce");
+      return VLCAL_ERR_UNSUPPORTED;
+    }
+    for (int i = 0; i < n_ctxs; i++) detached.push_back(ctxs[i]->p2p), ctxs[i]->p2p = nullptr;
   }
+  struct Reattach {
+    vlcal_nid_ctx* const* ctxs;
+    const std::vector<vlcal_p2p*>& px;
+    ~Reattach() {
+      for (size_t i = 0; i < px.size(); i++) ctxs[i]->p2p = px[i];
+    }
+  } reattach{ctxs, detached};
   PoseObjective obj;
   obj.ctxs = ctxs, obj.n_ctxs = n_ctxs, obj.init_T = init_T, obj.callback = callback, obj.allreduce = allreduce, obj.user = user;
 
@@ -204,12 +275,10 @@ int inner_solve_resident(
     ctx->profiling = profiling != 0;
     ctxs.v.push_back(ctx);
   }
-  if (g_default_p2p && g_default_p2p->device == device) {
-    // one bag per rank: every path can sum in-kernel; several local bags: only the persistent solve does
-    const bool pk_path = (g_solver_mode == 0 || g_solver_mode == 3) && pk_supported(ctxs.v.data(), static_cast<int>(ctxs.v.size()));
-    if (bags.size() == 1 || pk_path)
-      for (auto* c : ctxs.v) c->p2p = g_default_p2p;
-  }
+  // every context takes the default exchange, whatever this rank's bags: run_inner_solve then agrees on the path with the
+  // other ranks (agree_solve_path), which a rank deciding alone to solve without the exchange would leave waiting
+  if (g_default_p2p && g_default_p2p->device == device)
+    for (auto* c : ctxs.v) c->p2p = g_default_p2p;
   const double t_solve0 = now_ms();
   if (stats) stats->cull_ms += t_solve0 - t_cull0;
   vlcal_nm_result local;

@@ -47,6 +47,15 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line) {
   return VLCAL_ERR_CUDA;
 }
 
+unsigned long long sync_timeout_ns() {
+  static const unsigned long long v = [] {
+    const char* e = std::getenv("VLCAL_SYNC_TIMEOUT_MS");
+    const long long ms = e ? std::atoll(e) : 10000;  // a peer rank may enter its solve seconds later (upload / culling skew)
+    return static_cast<unsigned long long>(std::max(10LL, ms)) * 1000000ull;
+  }();
+  return v;
+}
+
 // ---------------------------------------------------------------------------------------------
 // camera factory rules + estimate_camera_fov
 // ---------------------------------------------------------------------------------------------
@@ -498,6 +507,7 @@ static void fill_common_args(vlcal_nid_ctx* ctx, NidArgs& a) {
     a.p2p_rank = ctx->p2p->rank;
     a.p2p_counter = ctx->p2p->d_counter;
     a.p2p_error = ctx->p2p->h_error;
+    a.p2p_timeout_ns = sync_timeout_ns();
   }
   a.ghist = ctx->d_ghist;
   a.counter = ctx->d_counter;
@@ -658,6 +668,55 @@ int nid_wait(vlcal_nid_ctx* ctx, double* nid_out, int32_t* hist_out) {
     }
     VL_CUDA(cudaStreamSynchronize(ctx->stream));  // the flag only orders the scores; histograms come from device memory
     VL_CUDA(cudaMemcpy(hist_out, ctx->d_hist_out, sizeof(int) * static_cast<size_t>(n_poses) * ctx->bins * ctx->bins, cudaMemcpyDeviceToHost));
+  }
+  return VLCAL_OK;
+}
+
+// every rank publishes one word and reads every rank's (p2p_gather)
+struct PeerGatherArgs {
+  P2PMailbox* box[P2P_MAX_RANKS];
+  int world, rank;
+  int* error;
+  unsigned long long* counter;
+  unsigned long long timeout_ns;
+  unsigned long long word;
+  unsigned long long* out;  // [world], mapped host memory
+};
+
+__global__ void __launch_bounds__(32) nid_peer_gather_kernel(const __grid_constant__ PeerGatherArgs a) {
+  __shared__ unsigned long long s_words[P2P_MAX_RANKS][8];
+  peer_exchange(a.box, a.world, a.rank, a.counter, a.error, a.timeout_ns, 1, [&](int) { return a.word; }, s_words);
+  if (threadIdx.x < a.world) a.out[threadIdx.x] = s_words[threadIdx.x][0];
+  __threadfence_system();
+}
+
+int p2p_gather(vlcal_p2p* p, cudaStream_t stream, unsigned long long word, unsigned long long* out) {
+  if (!p || !p->connected || p->world < 2) {
+    set_last_error("peer exchange is not connected");
+    return VLCAL_ERR_INVALID_ARGUMENT;
+  }
+  VL_CUDA(cudaSetDevice(p->device));
+  auto& pool = MemPool::instance();
+  void* h = nullptr;
+  VL_CUDA(pool.pinned_alloc(sizeof(unsigned long long) * P2P_MAX_RANKS, &h));
+  PeerGatherArgs a;
+  std::memset(&a, 0, sizeof(a));
+  for (int r = 0; r < p->world; r++) a.box[r] = p->peers[r];
+  a.world = p->world, a.rank = p->rank;
+  a.error = p->h_error;
+  a.counter = p->d_counter;
+  a.timeout_ns = sync_timeout_ns();
+  a.word = word;
+  a.out = static_cast<unsigned long long*>(h);
+  nid_peer_gather_kernel<<<1, 32, 0, stream>>>(a);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+  if (e == cudaSuccess) std::memcpy(out, h, sizeof(unsigned long long) * p->world);
+  pool.pinned_free(h);
+  if (e != cudaSuccess) return cuda_fail(e, "nid_peer_gather_kernel", __FILE__, __LINE__);
+  if (*p->h_error) {
+    set_last_error("peer exchange timed out: a rank died or the ranks are not solving in lockstep");
+    return VLCAL_ERR_CUDA;
   }
   return VLCAL_OK;
 }

@@ -153,6 +153,12 @@ int nid_ctx_create(
 int nid_evaluate_async(vlcal_nid_ctx* ctx, const double* T_colmajor, int n_poses, bool want_hist);
 int nid_wait(vlcal_nid_ctx* ctx, double* nid_out, int32_t* hist_out);
 
+// longest wait of any kernel for a peer rank's words: VLCAL_SYNC_TIMEOUT_MS (default 10 s, at least 10 ms)
+unsigned long long sync_timeout_ns();
+// one exchange of the connected exchange p (world > 1) on `stream`: this rank publishes `word`, out[r] receives rank r's
+// (all ranks must call it at the same point of their exchange sequence); returns after the words arrived
+int p2p_gather(vlcal_p2p* p, cudaStream_t stream, unsigned long long word, unsigned long long* out);
+
 // persistent cooperative kernel (nid_persistent.cu): can these contexts (bags of one camera on one device) run on it?
 bool pk_supported(vlcal_nid_ctx* const* ctxs, int n_ctxs);
 // a whole Nelder-Mead inner solve (visual_camera_calibration.cpp:103-129) in one launch; sums over the peer exchange

@@ -60,6 +60,7 @@ struct NidArgs {
   int* p2p_error;                  // mapped host word, set to 1 if a peer never answered
   unsigned long long* p2p_counter; // device word: number of exchanges done (advanced by the finalizing block of every
                                    // exchanging launch, so all ranks number their exchanges alike)
+  unsigned long long p2p_timeout_ns;  // longest wait for a peer's words (VLCAL_SYNC_TIMEOUT_MS, sync_timeout_ns)
   unsigned long long* timeline;    // optional [16] mapped host words: globaltimer stamps of the launch (vlcal_nid_debug_timeline)
   int* ghist;                 // [NID_MAX_POSES][nb] global accumulators, zero on entry, zero on exit
   unsigned int* counter;      // block ticket, zero on entry, zero on exit
@@ -210,46 +211,62 @@ __device__ __forceinline__ double warp_tree_sum(double v) {
   return v;
 }
 
-// called by the finalizing block after every pose's local score sits in a.nid_out (block-synchronised)
-static __device__ void nid_peer_allreduce(const NidArgs& a, int n_poses) {
+// One exchange over the round-1 mailboxes, run by one whole block: every rank sends n (<= 8) 64-bit words and receives
+// the n words of every rank, its own included: words[g][p] = rank g's word p.  The exchange number comes from the
+// exchange's device counter, which the round-1 kernels, the persistent kernel and the solve-path agreement
+// (nid_peer_gather_kernel) all advance, so every rank numbers its exchanges alike as long as all ranks run the same
+// sequence of them.  Thread t < n * world sends word(t % n) to rank t / n and then waits for that rank's word t % n; a
+// wait longer than timeout_ns (VLCAL_SYNC_TIMEOUT_MS) sets *error and leaves a stale word behind.
+template <typename Word>
+static __device__ void peer_exchange(
+  P2PMailbox* const* box, int world, int rank, unsigned long long* counter, int* error, unsigned long long timeout_ns, int n, Word word,
+  unsigned long long (*words)[8]) {
   __shared__ unsigned long long s_seq;
-  __shared__ double s_part[P2P_MAX_RANKS][8];
-  stamp(a, 10);
   const int t = threadIdx.x;
-  if (t == 0) s_seq = ++(*a.p2p_counter);  // every rank performs the same sequence of exchanges
+  if (t == 0) s_seq = ++(*counter);
   __syncthreads();
   const unsigned long long seq = s_seq;
   const int slot = static_cast<int>(seq & 1ull);
   const unsigned long long tag = ((seq & 0x7fffffffull) | 0x80000000ull) << 32;  // never 0 (the mailbox starts zeroed)
-  if (t < n_poses * a.p2p_world) {  // one thread per (peer, pose)
-    const int g = t / n_poses, p = t % n_poses;
-    {  // remote stores over NVLink: our partial sum -> rank g's mailbox
-      const unsigned long long bits = static_cast<unsigned long long>(__double_as_longlong(a.nid_out[p]));
-      volatile unsigned long long* dst = a.peer_box[g]->ll[a.p2p_rank][slot][p];
+  if (t < n * world) {  // one thread per (peer, word)
+    const int g = t / n, p = t % n;
+    {  // remote stores over NVLink: our word p -> rank g's mailbox
+      const unsigned long long bits = word(p);
+      volatile unsigned long long* dst = box[g]->ll[rank][slot][p];
       dst[0] = tag | (bits & 0xffffffffull);
       dst[1] = tag | (bits >> 32);
     }
-    {  // wait for rank g's partial sum of pose p to land in OUR mailbox
-      volatile unsigned long long* src = a.peer_box[a.p2p_rank]->ll[g][slot][p];
+    {  // wait for rank g's word p to land in OUR mailbox
+      volatile unsigned long long* src = box[rank]->ll[g][slot][p];
       const unsigned long long t0 = global_ns();
       unsigned int spins = 0;
       unsigned long long lo, hi;
       for (;;) {
         lo = src[0], hi = src[1];
         if ((lo & 0xffffffff00000000ull) == tag && (hi & 0xffffffff00000000ull) == tag) break;
-        if ((++spins & 1023u) == 0 && global_ns() - t0 > 2000000000ull) {  // 2 s: a peer died or fell out of lockstep
-          if (a.p2p_error) *a.p2p_error = 1;
+        if ((++spins & 1023u) == 0 && global_ns() - t0 > timeout_ns) {  // a peer died or fell out of lockstep
+          if (error) *error = 1;
           break;
         }
       }
-      s_part[g][p] = __longlong_as_double(static_cast<long long>((hi << 32) | (lo & 0xffffffffull)));
+      words[g][p] = (hi << 32) | (lo & 0xffffffffull);
     }
   }
   __syncthreads();
+}
+
+// called by the finalizing block after every pose's local score sits in a.nid_out (block-synchronised)
+static __device__ void nid_peer_allreduce(const NidArgs& a, int n_poses) {
+  __shared__ unsigned long long s_part[P2P_MAX_RANKS][8];
+  stamp(a, 10);
+  const int t = threadIdx.x;
+  peer_exchange(
+    a.peer_box, a.p2p_world, a.p2p_rank, a.p2p_counter, a.p2p_error, a.p2p_timeout_ns, n_poses,
+    [&](int p) { return static_cast<unsigned long long>(__double_as_longlong(a.nid_out[p])); }, s_part);
   stamp(a, 11);
   if (t < n_poses) {
     double total = 0.0;
-    for (int r = 0; r < a.p2p_world; r++) total += s_part[r][t];  // rank order: identical on every rank
+    for (int r = 0; r < a.p2p_world; r++) total += __longlong_as_double(static_cast<long long>(s_part[r][t]));  // rank order: identical on every rank
     a.nid_out[t] = total;
     if (a.nid_host) a.nid_host[t] = total;
   }

@@ -98,15 +98,6 @@ static int pk_geometry(int device, int num_sms, PkKernel kernel, int nb, int kpt
   return VLCAL_OK;
 }
 
-static unsigned long long pk_timeout_ns() {
-  static const unsigned long long v = [] {
-    const char* e = std::getenv("VLCAL_SYNC_TIMEOUT_MS");
-    const long long ms = e ? std::atoll(e) : 10000;  // a peer rank may enter its solve seconds later (upload / culling skew)
-    return static_cast<unsigned long long>(std::max(10LL, ms)) * 1000000ull;
-  }();
-  return v;
-}
-
 // Points per lane and tile (K).  Tiles are dealt to the warps round-robin, so K = 4 (128-point tiles) needs a cloud large
 // enough for several tiles per warp to stay balanced -- and there the lighter register footprint of K = 2 (768 threads per
 // SM without spills in the pose loop, one packed register pair per coordinate) measured faster anyway.  K = 4 remains as
@@ -198,7 +189,7 @@ void pk_fill_common(PkArgs& a, vlcal_nid_ctx* const* ctxs, int n_ctxs, const PkG
   a.box[0] = reinterpret_cast<PkMailbox*>(scratch + L.box);
   a.delta_stats = reinterpret_cast<unsigned long long*>(scratch + L.delta_stats);
   a.world = 1, a.rank = 0;
-  a.timeout_ns = pk_timeout_ns();
+  a.timeout_ns = sync_timeout_ns();
 }
 
 int pk_grid_size(const PkGeom& g, vlcal_nid_ctx* const* ctxs, int n_ctxs) {

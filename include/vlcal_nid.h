@@ -269,8 +269,10 @@ int vlcal_nid_p2p_create(int device, int rank, int world, vlcal_p2p** out, void*
 int vlcal_nid_p2p_connect(vlcal_p2p* px, const void* all_handles);
 int vlcal_nid_p2p_attach(vlcal_nid_ctx* ctx, vlcal_p2p* px); /* px == NULL detaches */
 void vlcal_nid_p2p_destroy(vlcal_p2p* px);
-/* contexts that vlcal_estimate_pose_nelder_mead / vlcal_calibrate_nelder_mead build internally attach this exchange when the
- * process passes exactly one bag (then the allreduce callback is not used); NULL clears it */
+/* contexts that vlcal_estimate_pose_nelder_mead / vlcal_calibrate_nelder_mead build internally attach this exchange; NULL
+ * clears it.  Before every solve on a connected exchange the ranks agree on the solve path (DESIGN.md section 7): ranks
+ * whose plans differ take the host loop together when each holds one bag, and otherwise all return
+ * VLCAL_ERR_UNSUPPORTED.  With several local bags and no persistent solve, an allreduce callback sums the host loop. */
 int vlcal_nid_p2p_set_default(vlcal_p2p* px);
 
 /* ---- view culling: ViewCulling::cull (src/vlcal/calib/view_culling.cpp:21-92) ------------
