@@ -215,12 +215,14 @@ def load_library():
     L.vlcal_turbo_colormap.argtypes = [vp]
     L.vlcal_colorize_points.argtypes = viewer + [C.c_float, vp, dp]
     L.vlcal_render_overlay.argtypes = viewer + [C.c_int, C.c_float, vp, vp, dp]
+    L.vlcal_agreement_map.argtypes = viewer + [C.c_int, C.c_int, C.c_float, dp, vp, vp, vp]
     L.vlcal_nm_default_params.argtypes = [C.POINTER(NMParams)]
     L.vlcal_nm_default_params.restype = None
     L.vlcal_nelder_mead_batched.argtypes = [C.c_int, NM_BATCH_FN, NM_OBSERVE_FN, vp, dp, C.POINTER(NMParams), C.POINTER(NMResult)]
     L.vlcal_calib_default_params.argtypes = [C.POINTER(CalibParams)]
     L.vlcal_calib_default_params.restype = None
     L.vlcal_estimate_pose_nelder_mead_ctx.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(CalibParams), dp, POSE_CALLBACK, ALLREDUCE_FN, vp, dp, C.POINTER(NMResult)]
+    L.vlcal_estimate_poses_nelder_mead_ctx.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(CalibParams), C.c_int, dp, vp, dp, C.POINTER(NMResult)]
     common = [C.c_int, C.c_int, dp, C.c_int, dp, C.c_int, C.POINTER(Bag), C.c_int, C.POINTER(CalibParams), dp, POSE_CALLBACK, ALLREDUCE_FN, vp, C.c_int, dp]
     L.vlcal_estimate_pose_nelder_mead.argtypes = common + [C.POINTER(NMResult), C.POINTER(CalibStats)]
     L.vlcal_calibrate_nelder_mead.argtypes = common + [C.POINTER(CalibStats)]

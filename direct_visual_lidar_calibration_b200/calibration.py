@@ -250,3 +250,28 @@ def estimate_pose_on_costs(costs, init_T_camera_lidar, params: VisualCameraCalib
         "num_evaluations": int(res.num_evaluations), "num_batches": int(res.num_batches), "num_evaluations_computed": int(res.num_evaluations_computed),
     }
     return colmajor_to_T(out)[0], r
+
+
+def estimate_poses_on_costs(costs, init_Ts, bag_mask=None, params: VisualCameraCalibrationParams | None = None):
+    """S independent Nelder-Mead solves over already-built CostCalculatorNID objects in ONE persistent launch: solve s
+    starts from init_Ts[s] and sums the costs b with bag_mask[s, b] (default: all), each exactly as
+    estimate_pose_on_costs([costs[b] for b in its bags], init_Ts[s], params) would run it.  Returns (T (S, 4, 4), list of
+    result dicts)."""
+    L = _lib.load_library()
+    params = params or VisualCameraCalibrationParams()
+    T0 = T_to_colmajor(init_Ts)
+    S = T0.shape[0]
+    mask = np.ones((S, len(costs)), dtype=np.uint8) if bag_mask is None else np.ascontiguousarray(np.asarray(bag_mask, dtype=bool).astype(np.uint8))
+    if mask.shape != (S, len(costs)):
+        raise ValueError(f"bag_mask must be ({S}, {len(costs)})")
+    handles = (C.c_void_p * len(costs))(*[c.handle for c in costs])
+    p = params.to_c()
+    out = np.empty((S, 16))
+    res = (_lib.NMResult * S)()
+    _lib.check(L.vlcal_estimate_poses_nelder_mead_ctx(handles, len(costs), C.byref(p), S, _dp(T0), mask.ctypes.data, _dp(out), res))
+    rs = [
+        {"converged": bool(r.converged), "num_iterations": int(r.num_iterations), "x": np.array(r.x[:6]), "y": float(r.y),
+         "num_evaluations": int(r.num_evaluations), "num_batches": int(r.num_batches), "num_evaluations_computed": int(r.num_evaluations_computed)}
+        for r in res
+    ]
+    return colmajor_to_T(out), rs

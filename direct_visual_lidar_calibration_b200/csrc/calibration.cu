@@ -452,6 +452,36 @@ int vlcal_estimate_pose_nelder_mead_ctx(
   return run_inner_solve(ctxs, n_ctxs, params, init_T_camera_lidar, callback, allreduce, user, T_out, nm_result);
 }
 
+int vlcal_estimate_poses_nelder_mead_ctx(
+  vlcal_nid_ctx* const* ctxs,
+  int n_ctxs,
+  const vlcal_calib_params* params,
+  int n_solves,
+  const double* init_T_camera_lidar,
+  const uint8_t* bag_mask,
+  double* T_out,
+  vlcal_nm_result* nm_results) {
+  if (!ctxs || n_ctxs < 1 || !params || n_solves < 1 || !init_T_camera_lidar || !bag_mask || !T_out || !nm_results || params->max_inner_iterations < 0) {
+    set_last_error("invalid arguments");
+    return VLCAL_ERR_INVALID_ARGUMENT;
+  }
+  for (int i = 0; i < n_ctxs; i++) {
+    if (!ctxs[i]) {
+      set_last_error("NULL context");
+      return VLCAL_ERR_INVALID_ARGUMENT;
+    }
+    if (ctx_exchange_is_fused(ctxs[i])) {
+      set_last_error("the solve axis is single-process: detach the peer exchange of every context");
+      return VLCAL_ERR_UNSUPPORTED;
+    }
+  }
+  if (!pk_supported(ctxs, n_ctxs)) {
+    set_last_error("several solves per launch need the persistent kernel (float clouds, lean classifier, bins <= 32, one camera, image size and device)");
+    return VLCAL_ERR_UNSUPPORTED;
+  }
+  return pk_solve_many(ctxs, n_ctxs, params, n_solves, init_T_camera_lidar, bag_mask, T_out, nm_results);
+}
+
 int vlcal_estimate_pose_nelder_mead(
   int device,
   int camera_model,

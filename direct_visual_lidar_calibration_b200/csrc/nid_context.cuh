@@ -167,6 +167,10 @@ bool pk_supported(vlcal_nid_ctx* const* ctxs, int n_ctxs);
 int pk_solve(
   vlcal_nid_ctx* const* ctxs, int n_ctxs, const vlcal_calib_params* params, const double init_T[16], vlcal_pose_callback callback, void* user, double T_out[16],
   vlcal_nm_result* nm_result, bool score_centroid);
+// n_solves independent solves of the kind pk_solve runs without a callback, in one launch: solve s from init_T[16 s] over
+// the contexts with bag_mask[s * n_ctxs + b] set (single process; every solve gets at least one block per bag)
+int pk_solve_many(
+  vlcal_nid_ctx* const* ctxs, int n_ctxs, const vlcal_calib_params* params, int n_solves, const double* init_T, const uint8_t* bag_mask, double* T_out, vlcal_nm_result* results);
 // sum over the contexts of calculate(T_p) for a pose list of any length, one launch (hist_out: bag 0's joint histograms)
 int pk_score_poses(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_colmajor, int n_poses, double* nid_out, int32_t* hist_out);
 

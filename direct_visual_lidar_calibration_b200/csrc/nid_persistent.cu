@@ -66,7 +66,7 @@ static std::map<std::tuple<int, const void*, size_t>, int> g_pk_occupancy;
 // Dynamic shared memory of one block: the histogram copies (whose space the finalizer reuses as staging), then the warps'
 // tile rings.  At 16 bins and K = 2: 48 KB of copies + 24 warps x 2 slots x 1 KB of rings = 96 KB, next to ~16 KB of
 // static PkShared -- within the 227 KB a block may opt in to on an H100.
-static int pk_geometry(int device, int num_sms, PkKernel kernel, int nb, int kpt, PkGeom* g) {
+static int pk_geometry(int device, int num_sms, const void* kernel, int nb, int kpt, PkGeom* g) {
   // histogram copies for 8 poses (the initial simplex of a 6-D solve is 7) -- two copies while they fit 64 KB
   const size_t per_copy = static_cast<size_t>(PK_MAX_POSES) * nb * sizeof(int);
   g->copies = static_cast<int>(std::max<size_t>(1, std::min<size_t>(PK_WARPS / 4, (64 * 1024) / per_copy)));  // one copy per four warps
@@ -76,7 +76,7 @@ static int pk_geometry(int device, int num_sms, PkKernel kernel, int nb, int kpt
   g->ring_off = static_cast<unsigned int>(tail);
   g->smem = tail + pk_ring_bytes(kpt);
   std::lock_guard<std::mutex> lock(g_pk_mu);
-  const auto key = std::make_tuple(device, reinterpret_cast<const void*>(kernel), g->smem);
+  const auto key = std::make_tuple(device, kernel, g->smem);
   auto it = g_pk_occupancy.find(key);
   if (it == g_pk_occupancy.end()) {
     int optin = 0;
@@ -213,7 +213,7 @@ int pk_solve(
   const PkKernel kernel = pk_pick(c0->cam.model, kpt, true);  // Nelder-Mead batches close in as the simplex shrinks
   PkGeom g;
   {
-    const int rc = pk_geometry(c0->device, c0->num_sms, kernel, c0->bins * c0->bins, pk_kernel_k(c0->cam.model, kpt), &g);
+    const int rc = pk_geometry(c0->device, c0->num_sms, reinterpret_cast<const void*>(kernel), c0->bins * c0->bins, pk_kernel_k(c0->cam.model, kpt), &g);
     if (rc != VLCAL_OK) return rc;
   }
   const int grid = pk_grid_size(g, ctxs, n_ctxs);
@@ -379,6 +379,152 @@ int pk_solve(
   return VLCAL_OK;
 }
 
+// ---- S independent Nelder-Mead solves in one launch (the solve axis) ----------------------------------------------------------
+
+static const void* pk_pick_solves(int model) {
+  switch (model) {
+    case CAM_PLUMB_BOB: return reinterpret_cast<const void*>(nid_persistent_solves_kernel<CAM_PLUMB_BOB>);
+    case CAM_FISHEYE: return reinterpret_cast<const void*>(nid_persistent_solves_kernel<CAM_FISHEYE>);
+    case CAM_ATAN: return reinterpret_cast<const void*>(nid_persistent_solves_kernel<CAM_ATAN>);
+    case CAM_OMNIDIR: return reinterpret_cast<const void*>(nid_persistent_solves_kernel<CAM_OMNIDIR>);
+    case CAM_EQUIRECTANGULAR: return reinterpret_cast<const void*>(nid_persistent_solves_kernel<CAM_EQUIRECTANGULAR, PK_DELTA_POSES != 0>);
+    case CAM_RATIONAL_POLYNOMIAL: return reinterpret_cast<const void*>(nid_persistent_solves_kernel<CAM_RATIONAL_POLYNOMIAL>);
+    default: return nullptr;
+  }
+}
+
+int pk_solve_many(
+  vlcal_nid_ctx* const* ctxs, int n_ctxs, const vlcal_calib_params* params, int n_solves, const double* init_T, const uint8_t* bag_mask, double* T_out, vlcal_nm_result* results) {
+  vlcal_nid_ctx* c0 = ctxs[0];
+  VL_CUDA(cudaSetDevice(c0->device));
+  if (n_solves > PK_MAX_SOLVES) {
+    set_last_error("solve axis: at most " + std::to_string(PK_MAX_SOLVES) + " solves per launch");
+    return VLCAL_ERR_UNSUPPORTED;
+  }
+  const void* kernel = pk_pick_solves(c0->cam.model);
+  const int nb = c0->bins * c0->bins;
+  PkGeom g;
+  {
+    const int rc = pk_geometry(c0->device, c0->num_sms, kernel, nb, 2, &g);
+    if (rc != VLCAL_OK) return rc;
+  }
+  // the bags of every solve, in context order (the order its scores are summed in)
+  std::vector<std::vector<vlcal_nid_ctx*>> bags(n_solves);
+  long long need = 0, want_sum = 0;
+  std::vector<long long> want(n_solves);
+  for (int s = 0; s < n_solves; s++) {
+    for (int b = 0; b < n_ctxs; b++)
+      if (bag_mask[static_cast<size_t>(s) * n_ctxs + b]) bags[s].push_back(ctxs[b]);
+    if (bags[s].empty()) {
+      set_last_error("solve " + std::to_string(s) + " includes no bag");
+      return VLCAL_ERR_INVALID_ARGUMENT;
+    }
+    want[s] = pk_grid_size(g, bags[s].data(), static_cast<int>(bags[s].size()));  // what a single solve of these bags takes
+    want_sum += want[s];
+    need += static_cast<long long>(bags[s].size());
+  }
+  // blocks: every solve what it would take alone while the device holds them all, otherwise in proportion to that, and at
+  // least one per bag of the solve
+  const long long total = std::min<long long>(want_sum, g.max_blocks);
+  if (need > total) {
+    set_last_error("solve axis: " + std::to_string(n_solves) + " solves need " + std::to_string(need) + " blocks (one per bag of each), the device runs " + std::to_string(g.max_blocks) +
+                   " co-resident blocks");
+    return VLCAL_ERR_UNSUPPORTED;
+  }
+  std::vector<int> share(n_solves);
+  long long assigned = 0;
+  for (int s = 0; s < n_solves; s++) {
+    share[s] = static_cast<int>(std::max<long long>(static_cast<long long>(bags[s].size()), want[s] * total / want_sum));
+    assigned += share[s];
+  }
+  while (assigned > total) {  // rounding up to the per-bag minimum can overshoot: take the excess from the largest shares
+    int k = -1;
+    for (int s = 0; s < n_solves; s++)
+      if (share[s] > static_cast<int>(bags[s].size()) && (k < 0 || share[s] > share[k])) k = s;
+    share[k]--, assigned--;
+  }
+  PkSolvesArgs m;
+  std::memset(&m, 0, sizeof(m));
+  m.n_groups = n_solves;
+  for (int s = 0; s < n_solves; s++) m.block_begin[s + 1] = m.block_begin[s] + share[s];
+  const int grid = m.block_begin[n_solves];
+
+  // device scratch: every solve's accumulators and counters (PkScratchLayout), then the group arguments; one memset
+  std::vector<size_t> off(n_solves + 1, 0);
+  for (int s = 0; s < n_solves; s++) off[s + 1] = off[s] + PkScratchLayout(static_cast<int>(bags[s].size()), nb).total;
+  const size_t args_off = off[n_solves];
+  DevBuf scratch;
+  scratch.device = c0->device;
+  VL_CUDA(MemPool::instance().device_alloc(c0->device, args_off + sizeof(PkArgs) * n_solves, &scratch.p));
+  char* sp = static_cast<char*>(scratch.p);
+  VL_CUDA(cudaMemsetAsync(sp, 0, args_off, c0->stream));
+
+  // host side: the outcomes (mapped pinned memory, written by each group's block 0), the error word, and the staging of
+  // the solves' initial states and the group arguments
+  const size_t res_bytes = (sizeof(PkResult) * n_solves + 64 + 255) & ~static_cast<size_t>(255);
+  const size_t stage_bytes = sizeof(PkSolve) * n_solves + sizeof(PkArgs) * n_solves + 64;
+  PinBuf host;
+  VL_CUDA(MemPool::instance().pinned_alloc(res_bytes + stage_bytes, &host.p));
+  char* hp = static_cast<char*>(host.p);
+  PkResult* h_results = reinterpret_cast<PkResult*>(hp);
+  int* h_error = reinterpret_cast<int*>(hp + sizeof(PkResult) * n_solves);
+  std::memset(hp, 0, res_bytes);
+  PkSolve* h_solves = reinterpret_cast<PkSolve*>(hp + res_bytes);
+  PkArgs* h_args = reinterpret_cast<PkArgs*>((reinterpret_cast<uintptr_t>(h_solves + n_solves) + 63) & ~static_cast<uintptr_t>(63));
+
+  NmParams nm;  // visual_camera_calibration.cpp:122-125, as pk_solve
+  nm.init_step = params->nelder_mead_init_step;
+  nm.convergence_var_thresh = params->nelder_mead_convergence_criteria;
+  nm.max_iterations = params->max_inner_iterations;
+  const double x0[6] = {0, 0, 0, 0, 0, 0};
+  for (int s = 0; s < n_solves; s++) {
+    const PkScratchLayout L(static_cast<int>(bags[s].size()), nb);
+    char* gs = sp + off[s];
+    std::memset(static_cast<void*>(&h_solves[s]), 0, sizeof(PkSolve));
+    h_solves[s].nm.begin(6, nm, x0, /*score_centroid=*/false);  // nobody observes the evaluations: as pk_solve without a callback
+    std::memcpy(h_solves[s].init_T, init_T + 16 * static_cast<size_t>(s), sizeof(h_solves[s].init_T));
+    VL_CUDA(cudaMemcpyAsync(gs + L.solve, &h_solves[s], sizeof(PkSolve), cudaMemcpyHostToDevice, c0->stream));
+    PkArgs& a = h_args[s];
+    pk_fill_common(a, bags[s].data(), static_cast<int>(bags[s].size()), g, share[s], gs, L);
+    a.solve = reinterpret_cast<const PkSolve*>(gs + L.solve);
+    a.result_host = &h_results[s];
+    a.error_host = h_error;
+    a.abort_flag = reinterpret_cast<unsigned int*>(sp + PkScratchLayout(static_cast<int>(bags[0].size()), nb).abort_flag);  // one for the launch
+  }
+  VL_CUDA(cudaMemcpyAsync(sp + args_off, h_args, sizeof(PkArgs) * n_solves, cudaMemcpyHostToDevice, c0->stream));
+  m.group = reinterpret_cast<const PkArgs*>(sp + args_off);
+  m.common = h_args[0];  // pk_supported: one camera, image size and bin count for every context
+
+  void* kargs[] = {&m};
+  VL_CUDA(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(PK_THREADS), kargs, g.smem, c0->stream));
+  VL_CUDA(cudaStreamSynchronize(c0->stream));
+  std::atomic_thread_fence(std::memory_order_acquire);
+  if (*h_error) {
+    set_last_error("persistent solves: a wait timed out (the grid was not co-resident)");
+    return VLCAL_ERR_CUDA;
+  }
+  for (int s = 0; s < n_solves; s++) {
+    const NmMachine& fin = h_results[s].nm;
+    double E[16];
+    host::se3_expmap_gtsam(fin.result_x, E);
+    host::isometry_mul(init_T + 16 * static_cast<size_t>(s), E, T_out + 16 * static_cast<size_t>(s));  // :129
+    vlcal_nm_result& r = results[s];
+    std::memset(&r, 0, sizeof(r));
+    r.converged = fin.converged;
+    r.num_iterations = fin.num_iterations;
+    for (int d = 0; d < 6; d++) r.x[d] = fin.result_x[d];
+    r.y = fin.result_y;
+    r.num_evaluations = fin.num_evaluations;
+    r.num_batches = fin.num_batches;
+    r.num_evaluations_computed = fin.num_evaluations_computed;
+    c0->passes += static_cast<int64_t>(h_results[s].batches);
+    c0->poses_total += static_cast<int64_t>(h_results[s].poses);
+  }
+  for (int i = 0; i < n_ctxs; i++) ctxs[i]->pk_last_kpt = 2;
+  c0->launches += 1;
+  return VLCAL_OK;
+}
+
 // ---- pose list ----------------------------------------------------------------------------------------------------------------
 
 int pk_score_poses(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_colmajor, int n_poses, double* nid_out, int32_t* hist_out) {
@@ -407,7 +553,7 @@ int pk_score_poses(vlcal_nid_ctx* const* ctxs, int n_ctxs, const double* T_colma
   PkKernel kernel = pk_pick(c0->cam.model, kpt, delta);
   PkGeom g;
   {
-    const int rc = pk_geometry(c0->device, c0->num_sms, kernel, c0->bins * c0->bins, pk_kernel_k(c0->cam.model, kpt), &g);
+    const int rc = pk_geometry(c0->device, c0->num_sms, reinterpret_cast<const void*>(kernel), c0->bins * c0->bins, pk_kernel_k(c0->cam.model, kpt), &g);
     if (rc != VLCAL_OK) return rc;
   }
   const int grid = pk_grid_size(g, ctxs, n_ctxs);

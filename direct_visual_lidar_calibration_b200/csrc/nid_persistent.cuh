@@ -1064,23 +1064,25 @@ __device__ __forceinline__ void pk_stamp(const PkArgs& a, unsigned long long bat
 // DPOSE: this instance carries the equirectangular delta step (instantiated for equirectangular, K = 2 only; the host
 // picks it for Nelder-Mead solves and for pose lists with a chunk inside the gate, see pk_pick).  Its anchor state costs
 // registers in the whole kernel, so the plain instance stays for everything else.
-template <int MODEL, int K, bool DPOSE = false>
-__global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __grid_constant__ PkArgs a) {
+// blk, grid: this block's index within the blocks that run the launch's work, and their number -- the whole grid for
+// nid_persistent_kernel, one solve's group for nid_persistent_solves_kernel
+template <int MODEL, int K, bool DPOSE>
+__device__ __forceinline__ void pk_run(const PkArgs& a, const PkArgs& grp, const unsigned int blk, const unsigned int grid) {
   extern __shared__ __align__(128) int smem_hist[];
   __shared__ PkShared sh;
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-  const bool solve_mode = a.solve != nullptr;
+  const bool solve_mode = grp.solve != nullptr;
 
   // block -> bag, warp -> its interleaved tiles of the bag's cloud
   int bag = 0;
-  while (bag + 1 < a.n_bags && static_cast<int>(blockIdx.x) >= a.bag[bag + 1].block_begin) bag++;
-  const PkBag& Bc = a.bag[bag];
+  while (bag + 1 < grp.n_bags && static_cast<int>(blk) >= grp.bag[bag + 1].block_begin) bag++;
+  const PkBag& Bc = grp.bag[bag];
   PkBagRegs B;
   B.points = Bc.points;
   B.bin_image = Bc.bin_image;
   const unsigned int bag_n = Bc.n, bag_block_begin = static_cast<unsigned int>(Bc.block_begin), bag_block_count = static_cast<unsigned int>(Bc.block_count);
   const unsigned int warps_total = bag_block_count * PK_WARPS;
-  const unsigned int warp_global = (blockIdx.x - bag_block_begin) * PK_WARPS + warp;
+  const unsigned int warp_global = (blk - bag_block_begin) * PK_WARPS + warp;
 
   PkWarp w;
   w.lane = lane;
@@ -1096,16 +1098,16 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
   // reads them back).  While a tile is scored it waits there instead of in registers live across the pose loop.
   constexpr bool DELTA = DPOSE && PK_DELTA_POSES && MODEL == CAM_EQUIRECTANGULAR && K % 2 == 0;  // as in pk_tile
   const unsigned int ring_state = static_cast<unsigned int>(__cvta_generic_to_shared(&sh.ring_state[warp]));
-  const int n_items_per_batch = a.n_bags * (solve_mode ? PK_MAX_POSES : a.chunk);  // finalizer items of a full pose-list chunk
-  const int fin_stride = max(1, static_cast<int>(gridDim.x) / (a.n_bags * PK_MAX_POSES));
+  const int n_items_per_batch = grp.n_bags * (solve_mode ? PK_MAX_POSES : grp.chunk);  // finalizer items of a full pose-list chunk
+  const int fin_stride = max(1, static_cast<int>(grid) / (grp.n_bags * PK_MAX_POSES));
 
   // ---- first batch ----
   if (solve_mode) {
     static_assert(sizeof(NmMachine) % 8 == 0, "NmMachine is copied as 8-byte words");
-    const unsigned long long* src = reinterpret_cast<const unsigned long long*>(&a.solve->nm);
+    const unsigned long long* src = reinterpret_cast<const unsigned long long*>(&grp.solve->nm);
     unsigned long long* dst = reinterpret_cast<unsigned long long*>(&sh.nm);
     for (int i = t; i < static_cast<int>(sizeof(NmMachine) / 8); i += PK_THREADS) dst[i] = src[i];
-    if (t < 16) sh.init_T[t] = a.solve->init_T[t];
+    if (t < 16) sh.init_T[t] = grp.solve->init_T[t];
     __syncthreads();
     if (warp == 0) {
       pk_poses_of_candidates(sh, sh.nm.n_cand, lane);
@@ -1113,14 +1115,14 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
     }
     if (t == 0) sh.n_poses = sh.nm.n_cand;
   } else {
-    const int pc = min(a.chunk, a.n_total);
-    if (t < pc) pk_pose_from_list(sh, t, a.poses_in + 12 * static_cast<size_t>(t));  // pc <= 8: warp 0
+    const int pc = min(grp.chunk, grp.n_total);
+    if (t < pc) pk_pose_from_list(sh, t, grp.poses_in + 12 * static_cast<size_t>(t));  // pc <= 8: warp 0
     if (DELTA && warp == 0) pk_delta_rows<K>(sh, pc, a.nb, lane);
     if (t == 0) sh.n_poses = pc;
   }
   for (int i = t; i < PK_MAX_POSES * 2 * PK_MAX_BINS; i += PK_THREADS) (&sh.bmarg[0][0])[i] = 0;
   if (t == 0) {
-    sh.seq_base = *a.seq_counter;
+    sh.seq_base = *grp.seq_counter;
     sh.trace_count = 0;
     sh.poses_scored = 0ull;
   }
@@ -1132,15 +1134,15 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
     // accumulator buffer of this batch: pose-list mode alternates two (each zeroed by its finalizers), Nelder-Mead mode
     // rotates three (every block reads all of them; buffer b is zeroed while batch b + 1 is finalized, see (B))
     const int buf = solve_mode ? static_cast<int>(batch % 3ull) : static_cast<int>(batch & 1ull);
-    if (blockIdx.x == 0 && t == 0) pk_stamp(a, batch, 0);
-    if (DELTA && blockIdx.x == 0 && t == 0 && sh.delta_on && a.delta_stats) a.delta_stats[0] += 1ull, a.delta_stats[1] += static_cast<unsigned long long>(n_poses);
+    if (blk == 0 && t == 0) pk_stamp(grp, batch, 0);
+    if (DELTA && blk == 0 && t == 0 && sh.delta_on && grp.delta_stats) grp.delta_stats[0] += 1ull, grp.delta_stats[1] += static_cast<unsigned long long>(n_poses);
     // pose-list mode runs ahead of the finalizers: buffer `buf` (accumulators, tile counter) must have been finalized for
     // chunk batch - 2 first.  (Nelder-Mead mode: seeing the scores of batch - 1 already implies it.)
     if (!solve_mode && batch >= 2) {
-      if (!pk_wait_counter(a, sh, a.fin_done + buf, static_cast<unsigned int>((batch >> 1) * static_cast<unsigned long long>(n_items_per_batch)))) return;
+      if (!pk_wait_counter(grp, sh, grp.fin_done + buf, static_cast<unsigned int>((batch >> 1) * static_cast<unsigned long long>(n_items_per_batch)))) return;
     }
-    const bool time_block = a.block_times != nullptr && batch == static_cast<unsigned long long>(a.block_times_batch) && t == 0;
-    if (time_block) a.block_times[4 * blockIdx.x + 0] = global_ns();
+    const bool time_block = grp.block_times != nullptr && batch == static_cast<unsigned long long>(grp.block_times_batch) && t == 0;
+    if (time_block) grp.block_times[4 * blk + 0] = global_ns();
     // Nelder-Mead mode, batch > 0: the histogram copies were zeroed and sh.tmax set while warp 0 stepped the simplex (end of
     // the previous batch), so the batch starts without a barrier
     const bool fresh = !solve_mode || batch == 0ull;
@@ -1173,7 +1175,7 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
       for (int i = t; i < a.copies * per_copy; i += PK_THREADS) smem_hist[i] = 0;
       __syncthreads();
     }
-    if (time_block) a.block_times[4 * blockIdx.x + 1] = global_ns();
+    if (time_block) grp.block_times[4 * blk + 1] = global_ns();
     for (;;) {
       const uint4 rs = lds_v4(ring_state);  // {tile, tiles left, step, slot}
       if (rs.y == 0u) break;
@@ -1199,12 +1201,12 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
       w.qn = 0;
       if (lane == 0) sts_u32(w.q_cnt, 0u);
     }
-    if (blockIdx.x == 0 && t == 0) pk_stamp(a, batch, 1);
+    if (blk == 0 && t == 0) pk_stamp(grp, batch, 1);
     __syncthreads();
-    if (time_block) a.block_times[4 * blockIdx.x + 2] = global_ns();
+    if (time_block) grp.block_times[4 * blk + 2] = global_ns();
     // ---- merge into the global accumulators -----------------------------------------------------------------------------
     {
-      int* g = a.ghist + (static_cast<size_t>(buf) * a.n_bags + bag) * PK_MAX_POSES * a.nb;
+      int* g = grp.ghist + (static_cast<size_t>(buf) * grp.n_bags + bag) * PK_MAX_POSES * a.nb;
       for (int k = t; k < per_copy; k += PK_THREADS) {
         int s = 0;
         for (int c = 0; c < a.copies; c++) s += smem_hist[c * per_copy + k];
@@ -1219,7 +1221,7 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
       }
       if (solve_mode) {
         __syncthreads();
-        int* gm = a.gmarg + (static_cast<size_t>(buf) * a.n_bags + bag) * PK_MAX_POSES * PK_MARG_STRIDE;
+        int* gm = grp.gmarg + (static_cast<size_t>(buf) * grp.n_bags + bag) * PK_MAX_POSES * PK_MARG_STRIDE;
         for (int i = t; i < n_poses * 2 * a.bins; i += PK_THREADS) {
           const int p = i / (2 * a.bins), f = i - p * 2 * a.bins;
           const int v = sh.bmarg[p][f];
@@ -1237,39 +1239,39 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
     __syncthreads();
     if (t == 0) {
       __threadfence();
-      atomicAdd(a.arrive + buf * PK_MAX_BAGS + bag, 1u);
+      atomicAdd(grp.arrive + buf * PK_MAX_BAGS + bag, 1u);
     }
-    if (blockIdx.x == 0 && t == 0) pk_stamp(a, batch, 2);
-    if (time_block) a.block_times[4 * blockIdx.x + 3] = global_ns();
+    if (blk == 0 && t == 0) pk_stamp(grp, batch, 2);
+    if (time_block) grp.block_times[4 * blk + 3] = global_ns();
     const unsigned long long seq = sh.seq_base + batch + 1ull;
     const int slot = static_cast<int>(seq & 1ull);
     const unsigned long long tag = ((seq & 0x7fffffffull) | 0x80000000ull) << 32;  // never 0 (mailboxes start zeroed)
     if (!solve_mode) {
       // ---- (B, pose list) finalize the (bag, pose) items this block owns; nobody waits for them but the chunk after next ----
-      for (int item = 0; item < a.n_bags * n_poses; item++) {
+      for (int item = 0; item < grp.n_bags * n_poses; item++) {
         const int ib = item / n_poses, ip = item % n_poses;
-        if (static_cast<int>((static_cast<long long>(ib * PK_MAX_POSES + ip) * fin_stride) % gridDim.x) != static_cast<int>(blockIdx.x)) continue;
-        const unsigned int expected = static_cast<unsigned int>(((batch >> 1) + 1ull) * static_cast<unsigned long long>(a.bag[ib].block_count));
-        if (!pk_wait_counter(a, sh, a.arrive + buf * PK_MAX_BAGS + ib, expected)) return;
-        if (item == 0 && t == 0) pk_stamp(a, batch, 3);
-        int* g = a.ghist + ((static_cast<size_t>(buf) * a.n_bags + ib) * PK_MAX_POSES + ip) * a.nb;
-        int* ho = (a.hist_out && ib == 0) ? a.hist_out + (static_cast<size_t>(batch) * a.chunk + ip) * a.nb : nullptr;
+        if (static_cast<int>((static_cast<long long>(ib * PK_MAX_POSES + ip) * fin_stride) % grid) != static_cast<int>(blk)) continue;
+        const unsigned int expected = static_cast<unsigned int>(((batch >> 1) + 1ull) * static_cast<unsigned long long>(grp.bag[ib].block_count));
+        if (!pk_wait_counter(grp, sh, grp.arrive + buf * PK_MAX_BAGS + ib, expected)) return;
+        if (item == 0 && t == 0) pk_stamp(grp, batch, 3);
+        int* g = grp.ghist + ((static_cast<size_t>(buf) * grp.n_bags + ib) * PK_MAX_POSES + ip) * a.nb;
+        int* ho = (grp.hist_out && ib == 0) ? grp.hist_out + (static_cast<size_t>(batch) * grp.chunk + ip) * a.nb : nullptr;
         const double nid = pk_block_nid(sh, g, a.nb, a.bins, ho, smem_hist);
         if (t == 0) {
           // sum over the launch's bags in bag order needs all of them; single-bag launches store directly
-          if (a.n_bags == 1) a.scores_out[batch * a.chunk + ip] = nid;
-          else a.scores_out[(batch * a.chunk + ip) * a.n_bags + ib] = nid;  // per-bag scores; the host adds them in order
+          if (grp.n_bags == 1) grp.scores_out[batch * grp.chunk + ip] = nid;
+          else grp.scores_out[(batch * grp.chunk + ip) * grp.n_bags + ib] = nid;  // per-bag scores; the host adds them in order
           __threadfence();
-          atomicAdd(a.fin_done + buf, 1u);
+          atomicAdd(grp.fin_done + buf, 1u);
         }
-        if (item == 0 && t == 0) pk_stamp(a, batch, 4);
+        if (item == 0 && t == 0) pk_stamp(grp, batch, 4);
         __syncthreads();
       }
       // ---- next chunk of the pose list (only the last chunk can be partial, and no merge ever waits for it) ----
-      const long long next0 = static_cast<long long>(batch + 1ull) * a.chunk;
-      const int pc = static_cast<int>(max(0ll, min(static_cast<long long>(a.chunk), static_cast<long long>(a.n_total) - next0)));
+      const long long next0 = static_cast<long long>(batch + 1ull) * grp.chunk;
+      const int pc = static_cast<int>(max(0ll, min(static_cast<long long>(grp.chunk), static_cast<long long>(grp.n_total) - next0)));
       __syncthreads();
-      if (t < pc) pk_pose_from_list(sh, t, a.poses_in + 12 * static_cast<size_t>(next0 + t));
+      if (t < pc) pk_pose_from_list(sh, t, grp.poses_in + 12 * static_cast<size_t>(next0 + t));
       if (DELTA && warp == 0) pk_delta_rows<K>(sh, pc, a.nb, lane);
       if (t == 0) sh.n_poses = pc;
       __syncthreads();
@@ -1282,21 +1284,21 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
     // Accumulators rotate over three buffers and are zeroed two batches ahead: buffer (batch + 2) % 3 was last read in
     // batch - 1 (finished by every block before it arrived here) and is next merged in batch + 2, which no block reaches
     // before every block arrived for batch + 1, i.e. after this block's zeroing (ordered by the arrival fence).
-    if (!pk_wait_arrivals(a, a.arrive + buf * PK_MAX_BAGS, static_cast<unsigned int>(batch / 3ull + 1ull))) return;
-    if (blockIdx.x == 0 && t == 0) pk_stamp(a, batch, 3);
+    if (!pk_wait_arrivals(grp, grp.arrive + buf * PK_MAX_BAGS, static_cast<unsigned int>(batch / 3ull + 1ull))) return;
+    if (blk == 0 && t == 0) pk_stamp(grp, batch, 3);
     {
-      const int nz = a.n_bags * PK_MAX_POSES * a.nb;
-      int* z = a.ghist + static_cast<size_t>((buf + 2) % 3) * nz;
-      for (int i = static_cast<int>(blockIdx.x) * PK_THREADS + t; i < nz; i += static_cast<int>(gridDim.x) * PK_THREADS) z[i] = 0;
-      const int nm = a.n_bags * PK_MAX_POSES * PK_MARG_STRIDE;
-      int* zm = a.gmarg + static_cast<size_t>((buf + 2) % 3) * nm;
+      const int nz = grp.n_bags * PK_MAX_POSES * a.nb;
+      int* z = grp.ghist + static_cast<size_t>((buf + 2) % 3) * nz;
+      for (int i = static_cast<int>(blk) * PK_THREADS + t; i < nz; i += static_cast<int>(grid) * PK_THREADS) z[i] = 0;
+      const int nm = grp.n_bags * PK_MAX_POSES * PK_MARG_STRIDE;
+      int* zm = grp.gmarg + static_cast<size_t>((buf + 2) % 3) * nm;
       // (from the last block down: the first blocks carry most of the joint accumulators)
-      for (int i = static_cast<int>(gridDim.x - 1u - blockIdx.x) * PK_THREADS + t; i < nm; i += static_cast<int>(gridDim.x) * PK_THREADS) zm[i] = 0;
+      for (int i = static_cast<int>(grid - 1u - blk) * PK_THREADS + t; i < nm; i += static_cast<int>(grid) * PK_THREADS) zm[i] = 0;
     }
     {
-      const int n_items = a.n_bags * n_poses;
-      const int* gbuf = a.ghist + static_cast<size_t>(buf) * a.n_bags * PK_MAX_POSES * a.nb;
-      const int* mbuf = a.gmarg + static_cast<size_t>(buf) * a.n_bags * PK_MAX_POSES * PK_MARG_STRIDE;
+      const int n_items = grp.n_bags * n_poses;
+      const int* gbuf = grp.ghist + static_cast<size_t>(buf) * grp.n_bags * PK_MAX_POSES * a.nb;
+      const int* mbuf = grp.gmarg + static_cast<size_t>(buf) * grp.n_bags * PK_MAX_POSES * PK_MARG_STRIDE;
       // items per round: what the dead histogram copies hold of staged terms, at most one item per warp
       const int round_items = min(PK_WARPS, (a.copies * PK_MAX_POSES * a.nb * 4) / pk_fin_item_bytes(a.nb, a.bins));
       for (int first = 0; first < n_items; first += round_items) {
@@ -1304,15 +1306,15 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
         pk_block_nid_items(gbuf, mbuf, first, count, n_poses, a.nb, a.bins, smem_hist, sh.fin_out);
         if (t < count) {
           const int item = first + t, ib = item / n_poses, ip = item - ib * n_poses;
-          const int word = (a.rank * a.n_bags + ib) * PK_MAX_POSES + ip;
+          const int word = (grp.rank * grp.n_bags + ib) * PK_MAX_POSES + ip;
           const double nid = sh.fin_out[t];
           sh.parts[word] = nid;
           // the other ranks get it from one block (NVLink peer stores, tagged words)
-          if (a.world > 1 && static_cast<unsigned int>(item) % gridDim.x == blockIdx.x) {
+          if (grp.world > 1 && static_cast<unsigned int>(item) % grid == blk) {
             const unsigned long long bits = static_cast<unsigned long long>(__double_as_longlong(nid));
-            for (int r = 0; r < a.world; r++) {
-              if (r == a.rank) continue;
-              volatile unsigned long long* dst = a.box[r]->w[slot][word];
+            for (int r = 0; r < grp.world; r++) {
+              if (r == grp.rank) continue;
+              volatile unsigned long long* dst = grp.box[r]->w[slot][word];
               dst[0] = tag | (bits & 0xffffffffull);
               dst[1] = tag | (bits >> 32);
             }
@@ -1320,13 +1322,13 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
         }
       }
     }
-    if (blockIdx.x == 0 && t == 0) pk_stamp(a, batch, 4);
+    if (blk == 0 && t == 0) pk_stamp(grp, batch, 4);
     // ---- (C) the other ranks' scores -> sum over ranks and bags -> Nelder-Mead step -> next poses ---------------------------
-    const int n_words = a.world * a.n_bags * n_poses;
+    const int n_words = grp.world * grp.n_bags * n_poses;
     bool timed_out = false;
-    if (a.world > 1 && t < n_words && t / (a.n_bags * n_poses) != a.rank) {
+    if (grp.world > 1 && t < n_words && t / (grp.n_bags * n_poses) != grp.rank) {
       const int src = t / n_poses, p = t % n_poses;  // src = rank * n_bags + bag
-      volatile unsigned long long* wsrc = a.box[a.rank]->w[slot][src * PK_MAX_POSES + p];
+      volatile unsigned long long* wsrc = grp.box[grp.rank]->w[slot][src * PK_MAX_POSES + p];
       const unsigned long long t0 = global_ns();
       unsigned int spins = 0;
       unsigned long long wl, wh;
@@ -1334,13 +1336,13 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
         wl = wsrc[0], wh = wsrc[1];
         if ((wl & 0xffffffff00000000ull) == tag && (wh & 0xffffffff00000000ull) == tag) break;
         if ((++spins & 255u) == 0) {
-          if (ld_acquire_u32(a.abort_flag) != 0u) {
+          if (ld_acquire_u32(grp.abort_flag) != 0u) {
             timed_out = true;
             break;
           }
-          if (global_ns() - t0 > a.timeout_ns) {
-            atomicExch(a.abort_flag, 1u);
-            if (a.error_host) *reinterpret_cast<volatile int*>(a.error_host) = 1;
+          if (global_ns() - t0 > grp.timeout_ns) {
+            atomicExch(grp.abort_flag, 1u);
+            if (grp.error_host) *reinterpret_cast<volatile int*>(grp.error_host) = 1;
             timed_out = true;
             break;
           }
@@ -1349,22 +1351,22 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
       sh.parts[src * PK_MAX_POSES + p] = __longlong_as_double(static_cast<long long>((wh << 32) | (wl & 0xffffffffull)));
     }
     if (__syncthreads_or(timed_out ? 1 : 0)) return;
-    if (blockIdx.x == 0 && t == 0) pk_stamp(a, batch, 5);
+    if (blk == 0 && t == 0) pk_stamp(grp, batch, 5);
     if (t < n_poses) {
       double total = 0.0;
-      for (int s = 0; s < a.world * a.n_bags; s++) total += sh.parts[s * PK_MAX_POSES + t];  // (rank, bag) order: identical everywhere
+      for (int s = 0; s < grp.world * grp.n_bags; s++) total += sh.parts[s * PK_MAX_POSES + t];  // (rank, bag) order: identical everywhere
       sh.ys[t] = total;
     }
     __syncthreads();
     if (warp == 0) {
       nm_warp_step(sh.nm, sh.ys, lane);
-      if (blockIdx.x == 0 && lane == 0) pk_stamp(a, batch, 7);
-      if (blockIdx.x == 0) {  // reference-order evaluations of this batch, for the callback replay on the host (posted writes)
+      if (blk == 0 && lane == 0) pk_stamp(grp, batch, 7);
+      if (blk == 0) {  // reference-order evaluations of this batch, for the callback replay on the host (posted writes)
         const int n_obs = sh.nm.n_obs;
         const int base = sh.trace_count;
         for (int k = 0; k < n_obs; k++) {
-          if (base + k < a.trace_cap) {
-            double* e = a.trace_host + static_cast<size_t>(base + k) * (NM_MAX_N + 1);
+          if (base + k < grp.trace_cap) {
+            double* e = grp.trace_host + static_cast<size_t>(base + k) * (NM_MAX_N + 1);
             if (lane < sh.nm.n) e[lane] = sh.nm.obs_x[k][lane];
             if (lane == 0) e[NM_MAX_N] = sh.nm.obs_y[k];
           }
@@ -1389,31 +1391,66 @@ __global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __g
       for (int i = t - 32; i < PK_MAX_POSES * 2 * PK_MAX_BINS; i += PK_THREADS - 32) (&sh.bmarg[0][0])[i] = 0;
     }
     __syncthreads();
-    if (blockIdx.x == 0 && t == 0) pk_stamp(a, batch, 6);
+    if (blk == 0 && t == 0) pk_stamp(grp, batch, 6);
   }
 
-  if (a.delta_stats && lane == 0) {
-    atomicAdd(a.delta_stats + 2, static_cast<unsigned long long>(sh.deferred[warp][0]));
-    atomicAdd(a.delta_stats + 3, static_cast<unsigned long long>(sh.deferred[warp][1]));
+  if (grp.delta_stats && lane == 0) {
+    atomicAdd(grp.delta_stats + 2, static_cast<unsigned long long>(sh.deferred[warp][0]));
+    atomicAdd(grp.delta_stats + 3, static_cast<unsigned long long>(sh.deferred[warp][1]));
   }
   // ---- results (block 0) ----
-  if (blockIdx.x == 0) {
+  if (blk == 0) {
     if (solve_mode) {
       const unsigned long long batches = static_cast<unsigned long long>(sh.nm.num_batches);
       const unsigned long long* src = reinterpret_cast<const unsigned long long*>(&sh.nm);
-      unsigned long long* dst = reinterpret_cast<unsigned long long*>(&a.result_host->nm);
+      unsigned long long* dst = reinterpret_cast<unsigned long long*>(&grp.result_host->nm);
       for (int i = t; i < static_cast<int>(sizeof(NmMachine) / 8); i += PK_THREADS) dst[i] = src[i];
       if (t == 0) {
-        a.result_host->batches = batches;
-        a.result_host->poses = sh.poses_scored;
-        a.result_host->trace_count = sh.trace_count;
-        *a.seq_counter = sh.seq_base + batches;  // every rank runs the same number of exchanges
+        grp.result_host->batches = batches;
+        grp.result_host->poses = sh.poses_scored;
+        grp.result_host->trace_count = sh.trace_count;
+        *grp.seq_counter = sh.seq_base + batches;  // every rank runs the same number of exchanges
       }
     }
     __threadfence_system();
     __syncthreads();
-    if (t == 0 && a.done_host && solve_mode) *reinterpret_cast<volatile unsigned long long*>(a.done_host) = a.done_seq;
+    if (t == 0 && grp.done_host && solve_mode) *reinterpret_cast<volatile unsigned long long*>(grp.done_host) = grp.done_seq;
   }
+}
+
+template <int MODEL, int K, bool DPOSE = false>
+__global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_kernel(const __grid_constant__ PkArgs a) {
+  pk_run<MODEL, K, DPOSE>(a, a, blockIdx.x, gridDim.x);
+}
+
+// ---- solve axis: S independent Nelder-Mead solves in one launch -------------------------------------------------------
+// The grid is cut into S groups of consecutive blocks; group s is a whole Nelder-Mead mode launch of its own -- its own
+// PkArgs (its bags, their block shares within the group, its PkSolve, its accumulators, arrival counters and result) --
+// and never waits for another group.  A solve's scores are functions of its integer histograms alone, which do not depend
+// on how many blocks share the cloud, so every solve follows the trajectory of a single-solve launch from the same start
+// on the same bags, bit for bit.  A group whose solve has finished leaves the kernel; the launch ends with the slowest.
+constexpr int PK_MAX_SOLVES = 64;
+
+struct PkSolvesArgs {
+  PkArgs common;                           // camera and image geometry, shared by every group (the hot loop reads it here)
+  const PkArgs* group;                     // [n_groups] in device memory
+  int n_groups;
+  int block_begin[PK_MAX_SOLVES + 1];      // group s: blocks [block_begin[s], block_begin[s + 1])
+};
+
+// K = 2 only: a solve's result does not depend on the points per lane, and every instance more costs compile time
+template <int MODEL, bool DPOSE = false>
+__global__ void __launch_bounds__(PK_THREADS, 1) nid_persistent_solves_kernel(const __grid_constant__ PkSolvesArgs m) {
+  // the group's arguments in shared memory, read outside the hot loop; the camera stays in the kernel parameter
+  __shared__ PkArgs ga;
+  int g = 0;
+  while (g + 1 < m.n_groups && static_cast<int>(blockIdx.x) >= m.block_begin[g + 1]) g++;
+  static_assert(sizeof(PkArgs) % 8 == 0, "PkArgs is copied as 8-byte words");
+  const unsigned long long* src = reinterpret_cast<const unsigned long long*>(m.group + g);
+  unsigned long long* dst = reinterpret_cast<unsigned long long*>(&ga);
+  for (int i = threadIdx.x; i < static_cast<int>(sizeof(PkArgs) / 8); i += PK_THREADS) dst[i] = src[i];
+  __syncthreads();
+  pk_run<MODEL, 2, DPOSE>(m.common, ga, blockIdx.x - static_cast<unsigned int>(m.block_begin[g]), static_cast<unsigned int>(m.block_begin[g + 1] - m.block_begin[g]));
 }
 
 // debug / test kernel: the lean classifier AND the exact path on every (point, pose); a.dbg: [0] point-poses,

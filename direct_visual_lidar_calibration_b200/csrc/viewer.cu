@@ -20,12 +20,12 @@
 
 #include "exact_classify.cuh"
 #include "preprocess_common.cuh"
+#include "turbo_blend.cuh"
 #include "turbo_colormap.hpp"
 
 namespace vlcal {
 
 static const unsigned char h_turbo_rgb[768] = {VLCAL_TURBO_RGB_BYTES};
-__constant__ unsigned char c_turbo_rgb[768] = {VLCAL_TURBO_RGB_BYTES};
 
 struct ViewerArgs {
   const void* points;  // float4 (x, y, z, intensity) or double4
@@ -40,24 +40,6 @@ struct ViewerArgs {
   const int* index_image;  // compose: [H*W]
   uint8_t* bgr;            // compose: [H*W*3]
 };
-
-__device__ __forceinline__ int turbo_index(float intensity) {
-  const double v = static_cast<double>(intensity) * 255.0;
-  if (!(v > 0.0)) return 0;  // negative, zero and NaN
-  return v >= 255.0 ? 255 : __double2int_rz(v);
-}
-
-// gray * w + turbo * (1 - w) per channel, alpha from 1 and 1 (points_color_updater.cpp:55-57)
-__device__ __forceinline__ float4 blend_colors(uint8_t pix, float intensity, float w, float one_minus_w) {
-  const float gray = __fmul_rn(__fdiv_rn(static_cast<float>(pix), 255.0f), w);
-  const unsigned char* t = c_turbo_rgb + 3 * turbo_index(intensity);
-  float4 c;
-  c.x = __fadd_rn(gray, __fmul_rn(__fdiv_rn(static_cast<float>(t[0]), 255.0f), one_minus_w));
-  c.y = __fadd_rn(gray, __fmul_rn(__fdiv_rn(static_cast<float>(t[1]), 255.0f), one_minus_w));
-  c.z = __fadd_rn(gray, __fmul_rn(__fdiv_rn(static_cast<float>(t[2]), 255.0f), one_minus_w));
-  c.w = __fadd_rn(w, one_minus_w);
-  return c;
-}
 
 template <int MODEL, bool F32>
 __global__ void __launch_bounds__(256) colorize_points_kernel(const __grid_constant__ ViewerArgs a) {
@@ -74,10 +56,6 @@ __global__ void __launch_bounds__(256) colorize_points_kernel(const __grid_const
   }
   const int pix = exact_pixel_hd<MODEL>(a.cam, a.cos_fov, a.width, a.height, a.pose, x, y, z);  // :41-52
   a.rgba[i] = pix < 0 ? make_float4(0.0f, 0.0f, 0.0f, 0.0f) : blend_colors(__ldg(a.image + pix), intensity, a.w, a.one_minus_w);
-}
-
-__device__ __forceinline__ uint8_t to_byte(float c) {
-  return static_cast<uint8_t>(min(max(__float2int_rn(__fmul_rn(c, 255.0f)), 0), 255));
 }
 
 template <bool F32>

@@ -58,3 +58,19 @@ def render_overlay(proj: GenericCamera, image, T_camera_lidar, points, intensiti
     args = _viewer_args(proj, data, T_camera_lidar, device)
     _lib.check(_lib.load_library().vlcal_render_overlay(*args, int(point_radius), float(np.float32(blend_weight)), bgr.ctypes.data, index.ctypes.data, C.byref(ms)))
     return (bgr, index, ms.value) if return_kernel_ms else (bgr, index)
+
+
+def agreement_map(proj: GenericCamera, image, T_camera_lidar, points, intensities, bins: int = 16, point_radius: int = 1, blend_weight: float = 0.7, device: int = -1):
+    """Where the LiDAR and the camera disagree at T_camera_lidar -> (pointwise mutual information per point (N,) float64,
+    NaN where the NID histogram does not count the point; joint histogram (bins, bins) [image_bin, lidar_bin] int32, as
+    CostCalculatorNID.calculate_batch returns it; BGR uint8 (H, W, 3); winning point per pixel int32 (H, W)).  The image is
+    the overlay of render_overlay with turbo(0.5 + PMI / 4) in place of turbo(intensity)."""
+    data = VisualLiDARData(image, points, intensities)
+    h, w = data.image.shape
+    pmi = np.empty(data.size())
+    hist = np.empty(bins * bins, dtype=np.int32)
+    bgr = np.empty((h, w, 3), dtype=np.uint8)
+    index = np.empty((h, w), dtype=np.int32)
+    args = _viewer_args(proj, data, T_camera_lidar, device)
+    _lib.check(_lib.load_library().vlcal_agreement_map(*args, int(bins), int(point_radius), float(np.float32(blend_weight)), _dp(pmi), hist.ctypes.data, bgr.ctypes.data, index.ctypes.data))
+    return pmi, hist.reshape(bins, bins).T.copy(), bgr, index

@@ -402,6 +402,37 @@ int vlcal_render_overlay(
   int32_t* index_image_out,
   double* kernel_ms_out);
 
+/* Agreement map at T_camera_lidar: per point, the pointwise mutual information log(p(a,b) / (p(a) p(b))) of its joint bin
+ * (image bin a, LiDAR bin b) in the NID histogram of the pose, computed as log(c_ab * N / (c_a * c_b)) from the integer
+ * counts; the histogram is calculate's (same decision per point, same bins, same FoV).  pmi_out: [n_points], NaN for a
+ * point the histogram does not count.  hist_out (may be NULL): [bins * bins] at image_bin + lidar_bin * bins, as
+ * vlcal_nid_evaluate's hist_out.  bgr_out / index_image_out: as vlcal_render_overlay, with the winner's colour
+ * turbo(0.5 + PMI / (2 * VLCAL_AGREEMENT_PMI_RANGE)) in place of turbo(intensity): red where the point's bin pair is more
+ * frequent than chance (the LiDAR and the camera agree), blue where it is rarer.  bins in [1, 32]. */
+#define VLCAL_AGREEMENT_PMI_RANGE 2.0
+int vlcal_agreement_map(
+  int device,
+  int camera_model,
+  const double* intrinsics,
+  int n_intrinsics,
+  const double* distortion,
+  int n_distortion,
+  int width,
+  int height,
+  const uint8_t* image,
+  int row_stride,
+  const double T_camera_lidar[16],
+  const double* points_xyzw,
+  const double* intensities,
+  int64_t n_points,
+  int bins,
+  int point_radius,
+  float blend_weight,
+  double* pmi_out,
+  int32_t* hist_out,
+  uint8_t* bgr_out,
+  int32_t* index_image_out);
+
 /* ---- solver surface ------------------------------------------------------------------ */
 
 /* how vlcal_estimate_pose_nelder_mead* / vlcal_calibrate_nelder_mead iterate (process-wide):
@@ -514,6 +545,26 @@ int vlcal_estimate_pose_nelder_mead_ctx(
   void* user,
   double T_out[16],
   vlcal_nm_result* nm_result);
+
+/* n_solves independent inner solves of vlcal_estimate_pose_nelder_mead_ctx (no callback, no all-reduce) in ONE launch of
+ * the persistent kernel: solve s starts from init_T_camera_lidar[16 s .. 16 s + 15] (T = init_T_s * Expmap(x), x0 = 0)
+ * and sums the contexts b with bag_mask[s * n_ctxs + b] != 0, in context order.  Each solve takes exactly the
+ * trajectory a single-solve call from the same start over the same contexts takes (same simplex, iterations, result,
+ * bit for bit).  T_out: [n_solves][16]; nm_results: [n_solves].
+ * VLCAL_ERR_UNSUPPORTED: the contexts cannot run on the persistent kernel (double-layout cloud, bins > 32, ...), one of
+ * them has a multi-rank peer exchange attached (the solve axis is single-process), n_solves > 64, or the device cannot
+ * hold one block per included bag of every solve at once.  The solves always run on the persistent kernel, whatever
+ * vlcal_nid_set_solver_mode selects for single solves, and record no profiling events (vlcal_nid_get_profile counts the
+ * launch, its passes and poses, not its time). */
+int vlcal_estimate_poses_nelder_mead_ctx(
+  vlcal_nid_ctx* const* ctxs,
+  int n_ctxs,
+  const vlcal_calib_params* params,
+  int n_solves,
+  const double* init_T_camera_lidar,
+  const uint8_t* bag_mask,
+  double* T_out,
+  vlcal_nm_result* nm_results);
 
 /* VisualCameraCalibration::estimate_pose_nelder_mead (visual_camera_calibration.cpp:70-139) from host data:
  * view culling at init_T (GPU), one cost context per bag, Nelder-Mead, pose out. */
